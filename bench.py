@@ -5,6 +5,7 @@
     python bench.py --gpus N --steps K --warmup W            # this implementation (one rank per GPU under torchrun)
     python bench.py --impl reference --steps K --warmup W    # the reference's own CPU code on the host cores
     python bench.py --config c5 --gpus 8                     # BASELINE configs[4] as the headline of the line instead of configs[1]
+    python bench.py --gpus 1 --steps K --dump-outputs DIR    # also write the film of the last timed step to DIR (see dump_outputs)
 
 One "step" = one complete render of the workload (all pixels x all samples of this rank's shard) + the film reduce.
 N > 1, headline (`value`): weak scaling -- every rank renders its own 1024 sample indices of every pixel (rank r: [r*1024, (r+1)*1024)
@@ -48,7 +49,7 @@ def measured_peaks():
             return json.load(open(p)), "measured"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0}, "fallback"
+    return {"hbm_gbs": 3350.0}, "H100 SXM data sheet"
 
 
 def usable_cores():
@@ -73,7 +74,7 @@ def usable_cores():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown," \
         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -111,6 +112,37 @@ class ClockSampler:
         if not sm:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": [], "samples": 0}
         return {"sm_mhz": float(np.median(sm)), "sm_max_mhz": float(max(mx)), "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def gpu_info(gpu_index=0):
+    """Name, power limit and maximum SM clock of the card: part of every number measured on it."""
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", str(gpu_index)],
+                           capture_output=True, text=True, timeout=30)
+        name, power, clock = [c.strip() for c in r.stdout.strip().split(",")]
+        return {"name": name, "power_limit_w": float(power), "sm_max_mhz": float(clock)}
+    except Exception:
+        import torch
+        return {"name": torch.cuda.get_device_name(gpu_index), "power_limit_w": None, "sm_max_mhz": None}
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, film):
+    """Writes what the timed path returned in its last step: the (H, W, 5) film of b2_render (RGB, alpha, filter weight), float32, as
+    out_dir/film.npy.  A film above DUMP_BYTES is replaced by a fixed, seeded sample of its pixels (film_sample.npy, (n, 5)) and their
+    row-major pixel indices (pixel_index.npy, float64), so that two builds can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    film = np.ascontiguousarray(film, np.float32)
+    if film.nbytes <= DUMP_BYTES:
+        np.save(os.path.join(out_dir, "film.npy"), film)
+        return
+    flat = film.reshape(-1, film.shape[-1])
+    n = DUMP_BYTES // (flat.shape[1] * 4 + 8)
+    idx = np.sort(np.random.default_rng(0).choice(flat.shape[0], n, replace=False))
+    np.save(os.path.join(out_dir, "film_sample.npy"), flat[idx])
+    np.save(os.path.join(out_dir, "pixel_index.npy"), idx.astype(np.float64))
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -282,10 +314,9 @@ def run_reference(args):
 # ------------------------------------------------------------------------------------------------------------------------------
 def traversal_metric(ctx, hbm_gbs, n_inst=100, n_rays=1 << 22):
     """Second half of BASELINE's metric ("traversal HBM GB/s vs peak"): the closest-hit traversal kernel on the FLATTENED 10 M-triangle
-    scene (1.1 GB of nodes + triangles: cannot sit in the 126 MB L2), incoherent rays from the bounding sphere (kdbench-style origins,
-    src/utils/kdbench.cpp:222-229) aimed at random mesh vertices.  Reported: Grays/s, the algorithmic bytes the kernel's own counters
-    imply, and -- per SURVEY.md 8d -- the DRAM bytes ncu measured for this very launch (profiles/r02_ncu_traversal.json) over the
-    live duration."""
+    scene (1.1 GB of nodes + triangles: cannot sit in the 50 MB L2), incoherent rays from the bounding sphere (kdbench-style origins,
+    src/utils/kdbench.cpp:222-229) aimed at random mesh vertices.  Reported: Grays/s and the algorithmic bytes the kernel's own counters
+    imply over the live duration."""
     import torch
     from mitsuba_b200 import api
     from mitsuba_b200.scene import stress_scene
@@ -317,16 +348,6 @@ def traversal_metric(ctx, hbm_gbs, n_inst=100, n_rays=1 << 22):
     res = {"scene": f"stress {n_inst}x100k = {d.n_triangles()} triangles flattened, {st['n_bvh_nodes']} BVH nodes of {node_b} B", "rays": n_rays,
            "kernel": "k_trace_rays (closest hit)", "mrays_s": n_rays / ms / 1e3, "ms": ms, "node_visits_per_ray": nv, "tri_tests_per_ray": pt,
            "algorithmic_gbs": alg / ms / 1e6, "unit": "GB/s", "peak": hbm_gbs, "algorithmic_frac": alg / ms / 1e6 / hbm_gbs, "commit_s": commit_s}
-    tp = os.path.join(ROOT, "profiles", "r02_ncu_traversal.json")
-    if os.path.exists(tp):
-        try:
-            nc = json.load(open(tp))
-            res["dram_bytes_per_launch_ncu"] = nc["dram_bytes"]
-            res["achieved"] = nc["dram_bytes"] / ms / 1e6   # ncu's DRAM bytes of the same launch over the live duration
-            res["frac"] = res["achieved"] / hbm_gbs
-            res["lanes_per_instruction_ncu"] = nc.get("lanes_per_instruction")
-        except Exception:
-            pass
     sc.close()
     return res
 
@@ -398,6 +419,7 @@ def main():
     ap.add_argument("--no-configs", action="store_true", help="skip the c3 / c4 / c5 side measurements")
     ap.add_argument("--no-volpath", action="store_true", help="(kept for scripts) same as --no-configs")
     ap.add_argument("--no-traversal", action="store_true", help="skip the isolated BVH-traversal measurement (10 M triangles)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the film of the last timed step to DIR (rank 0)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -515,6 +537,8 @@ def main():
     value = samples_per_step / (ms_step / 1e3) / 1e6
     pool = scene.stats()["pool_size"]
     film_host = film.cpu().numpy() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, film_host)
 
     # ---- e2e: through the C-ABI with host buffers (scene commit + render into a host film), same metric, same number of steps ----
     host_film = torch.zeros((H, W, 5), dtype=torch.float32).pin_memory()   # the step's result is read back into pinned host memory
@@ -604,13 +628,6 @@ def main():
                     "generate": (4 + 4 + 4 + 16 + 8) + 2 * 20 + (32 + 32 + 8 + 8 + 4 + 4)}[dom]
         items = {"extend": rays, "occluded": shadow, "shade": rays, "generate": smp}[dom] / n_dom
         achieved = per_item * items / (avg_ms / 1e3) / 1e9 if avg_ms > 0 else 0.0
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(tp):
-            try:
-                traffic = json.load(open(tp)).get("k_" + dom)
-            except Exception:
-                pass
         line = {
             "metric": "Msamples/sec Cornell box 1024spp" if args.config == "c2" else f"Msamples/sec BASELINE config {args.config}", "value": value, "unit": "Msamples/s",
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True,
@@ -619,13 +636,14 @@ def main():
                                     f"BASELINE {args.config}: {W}x{H} @ {total_spp} spp in total"),
                        **(WORKLOAD if args.config == "c2" else {}), "spp_per_gpu": (hi - lo), "spp_total": total_spp, "width": W, "height": H,
                        "parallelism": f"sample-index sharding x{world}, 1 film reduce", "pool_size": int(pool),
-                       "l2": "path pool + film (%.0f MB) exceed the 126 MB L2; every iteration re-streams them" % ((pool * (64 + 16 + 8 + 8 + 8 + 48 + 8) + W * H * 20) / 1e6),
+                       "l2": "path pool + film (%.0f MB) exceed the 50 MB L2; every iteration re-streams them" % ((pool * (64 + 16 + 8 + 8 + 8 + 48 + 8) + W * H * 20) / 1e6),
                        "fp": "parity (-fmad=false)" if args.parity else "fast (FMA contraction, --use_fast_math)", "commit_s": commit_s},
             "e2e": e2e,
             "gpu_launches": int(agg["launches"]),
             "clocks": clock_info,
+            "gpu": gpu_info(local),
             "roofline": {"bound": "hbm", "kernel": "k_" + dom, "achieved": achieved, "peak": peaks.get("hbm_gbs"), "unit": "GB/s",
-                         "frac": achieved / peaks.get("hbm_gbs", 1.0), "traffic": traffic, "peak_source": which + " (MEASURED_PEAKS.json hbm_gbs)",
+                         "frac": achieved / peaks.get("hbm_gbs", 1.0), "peak_source": which,
                          "avg_launch_ms": avg_ms, "avg_launch_ms_cuda_events": ev_check["" + dom] if ev_check else None,
                          "timer": "%globaltimer stamps inside the kernels (max CTA end - min CTA start per launch), timed region runs as one CUDA graph per iteration; cross-checked by an untimed step with CUDA events around plain launches",
                          "share_of_step": shares[dom] / max(1e-9, sum(shares.values())),
@@ -646,7 +664,7 @@ def main():
             line["configs"] = configs
         if not args.no_traversal:
             try:
-                line["traversal"] = traversal_metric(ctx, peaks.get("hbm_gbs", 6650.0))
+                line["traversal"] = traversal_metric(ctx, peaks.get("hbm_gbs", 3350.0))
             except Exception as e:
                 line["traversal"] = {"error": str(e)}
         if not args.no_configs and args.config == "c2" and full_size and world == 1:

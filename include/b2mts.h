@@ -1,4 +1,4 @@
-/* b2mts.h -- C-ABI of the B200-native wavefront path tracer that stands in for Mitsuba 0.6's
+/* b2mts.h -- C-ABI of the H100 (sm_90a) wavefront path tracer that stands in for Mitsuba 0.6's
  * `path` integrator hot path.  Plain C: opaque handles, pointers and sizes; no C++ or torch types.
  *
  * Every entry point names the reference interface it replaces (paths relative to the Mitsuba 0.6

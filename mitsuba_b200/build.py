@@ -1,4 +1,4 @@
-"""Builds libb2mts.so (CUDA kernels for sm_100a + the C-ABI) in-tree with nvcc.
+"""Builds libb2mts.so (CUDA kernels for sm_90a + the C-ABI) in-tree with nvcc.
 
     python -m mitsuba_b200.build [--force]
 
@@ -18,7 +18,7 @@ HOST = os.path.join(HERE, "host")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "libb2mts.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-ffp-contract=off,-fno-fast-math", "-I", os.path.join(HERE, "..", "include")]
 
 UNITS = [

@@ -178,7 +178,7 @@ struct b2_scene {
 // ------------------------------------------------------------------------------------------------
 // lifetime
 // ------------------------------------------------------------------------------------------------
-extern "C" const char *b2_version(void) { return "b2mts 0.1 (sm_100a wavefront path tracer)"; }
+extern "C" const char *b2_version(void) { return "b2mts 0.1 (sm_90a wavefront path tracer)"; }
 extern "C" int b2_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;
@@ -227,9 +227,9 @@ extern "C" int b2_context_create(int device, b2_ctx **out) {
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
     ctx->numSMs = prop.multiProcessorCount;
-    if (prop.major < 10) {
+    if (prop.major != 9 || prop.minor != 0) { // sm_90a code runs on compute capability 9.0 only
         delete ctx->store; delete ctx;
-        return fail(nullptr, B2_ERR_NO_DEVICE, "device is not sm_100 class; kernels are built for sm_100a only");
+        return fail(nullptr, B2_ERR_NO_DEVICE, "device is not compute capability 9.0; kernels are built for sm_90a only");
     }
     if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) { delete ctx->store; delete ctx; return fail(nullptr, B2_ERR_CUDA, "stream create failed"); }
     // Sobol tables
@@ -1404,8 +1404,8 @@ static int fillRender(b2_scene *s, const b2_render_params *p, DRender &r) {
     // never consumed by a pixel outside the film (workItemPixel in b2_kernels.inl).
     r.tilesX = (uint32_t) s->W / 8; r.tilesY = (uint32_t) s->H / 8;
     { // samples per tile visit: the largest divisor of the sample count that does not exceed B2_ROUND_SPP (0 = all samples at once).
-      // Measured on B200, Cornell 1024^2 @ 256 spp, Msamples/s: box filter 1646 / 1633 / 1619 / 1585 and gaussian 1229 / 1387 / 1455 /
-      // 1464 for all / 64 / 16 / 4 samples per round: a 5 x 5 splat wants the in-flight paths spread over many pixels, a 1-pixel one does not.
+      // A 5 x 5 gaussian splat wants the in-flight paths spread over many pixels (the L2 serialises atomics per address), a 1-pixel box
+      // splat does not.
         const uint32_t nS = (uint32_t) (r.sampleHi - r.sampleLo);
         uint32_t want = p->rfilter == B2_RFILTER_GAUSSIAN ? 8 : 0;
         if (const char *e = getenv("B2_ROUND_SPP")) want = (uint32_t) atoi(e);
@@ -1482,16 +1482,16 @@ extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
     if (rc) return rc;
     // Which kernel set renders?  parity_mode 1: the IEEE build (-fmad=false, accurate division / sqrt / sincos, TriAccel).  parity_mode 0: the
     // throughput build -- EXCEPT for `path` renders of scenes with a transmissive BSDF.  A path that bounces inside a glass ball amplifies
-    // ulp-level differences chaotically: under FMA contraction alone 3e-5 of such paths leave the reference's path (profiles/
-    // r02_flip_trace.json: different hit, other lobe, other ending -- not fast-math, not the plane-form triangle test), each an unrelated
-    // sample of a heavy-tailed estimator, i.e. 1.2e-3 relative L2 at 1024^2 @ 512 spp whatever else the kernels do.  Shading such scenes
+    // ulp-level differences chaotically: under FMA contraction alone a few in 1e5 of such paths leave the reference's path (different hit,
+    // other lobe, other ending -- not fast-math, not the plane-form triangle test), each an unrelated sample of a heavy-tailed estimator,
+    // i.e. above 1e-3 relative L2 at 1024^2 @ 512 spp whatever else the kernels do.  Shading such scenes
     // with the IEEE kernels and keeping only the traversal fast ("hybrid", tried: exact TriAccel (t,u,v) of the winning triangle) removes
     // a third of the flips -- the fast traversal still picks the neighbouring triangle at shared edges -- so those scenes get the IEEE
-    // build as a whole; it costs 7 % on BASELINE config 3 (BVH traversal dominates there).  flags bit8 forces the throughput kernels.
+    // build as a whole (BVH traversal dominates BASELINE config 3, so the IEEE shading costs little there).  flags bit8 forces the throughput kernels.
     const bool autoIeee = s->hasTransmission && p->integrator == B2_INTEGRATOR_PATH && !(p->flags & 256);
     const bool parityMode = p->parity_mode != 0 || autoIeee;
     const LaunchCfg &cfg = parityMode ? s->cfgParity : s->cfgFast;
-    uint32_t Q = p->pool_size > 0 ? (uint32_t) p->pool_size : (1u << 22); // 4M paths: measured sweet spot on B200 (DESIGN.md)
+    uint32_t Q = p->pool_size > 0 ? (uint32_t) p->pool_size : (1u << 22); // 4M paths (~0.6 GB)
     Q = std::max<uint32_t>(Q, 1024u);
     Q = (uint32_t) std::min<uint64_t>(Q, std::max<uint64_t>(1024u, r.totalWork));
     Q = (Q + 255u) & ~255u;

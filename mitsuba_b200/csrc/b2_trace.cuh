@@ -138,29 +138,18 @@ B2_DEV bool boxHit(float bx0, float by0, float bz0, float bx1, float by1, float 
 // Throughput build: the list holds paired records (b2_host.cpp "flat leaf of the throughput build"): a coplanar pair of
 // triangles costs one plane test + one hit point; a parallelogram additionally shares (u, v).
 //
-// Blackwell: a scalar FFMA issues every second cycle per scheduler, the packed FFMA2 (PTX fma.rn.f32x2, one instruction = two
-// FP32 FMAs on a 64-bit register pair) is what reaches the full FP32 rate.  The kernels that run this loop are FP32-issue bound
-// (ncu: 70-77 % issue active), so the leaf is stored TWO RECORDS WIDE: element k of record 2j sits next to element k of record
-// 2j + 1, one packed instruction evaluates both, and the ray is kept duplicated in register pairs.  Odd counts are padded with a
-// record that can never be hit (N = 0, d0 = -1: t = -inf).
+// The leaf is stored TWO RECORDS WIDE: element k of record 2j sits next to element k of record 2j + 1, so one float4 load
+// feeds the same step of two records and the two independent FMA chains interleave (the loop is FP32-issue bound).  Odd
+// counts are padded with a record that can never be hit (N = 0, d0 = -1: t = -inf).  Hopper has no packed FP32 arithmetic:
+// each pair operation is two scalar round-to-nearest, flush-to-zero instructions (the same rounding element by element as
+// a packed f32x2 instruction would give).
 struct F2 { float x, y; };
-B2_DEV unsigned long long f2bits(const F2 &a) { return ((unsigned long long) __float_as_uint(a.y) << 32) | __float_as_uint(a.x); }
-B2_DEV F2 f2from(unsigned long long v) { F2 r; r.x = __uint_as_float((uint32_t) v); r.y = __uint_as_float((uint32_t) (v >> 32)); return r; }
-B2_DEV F2 fma2(const F2 &a, const F2 &b, const F2 &c) {
-    unsigned long long r;
-    asm("fma.rn.ftz.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(f2bits(a)), "l"(f2bits(b)), "l"(f2bits(c)));
-    return f2from(r);
-}
-B2_DEV F2 mul2(const F2 &a, const F2 &b) {
-    unsigned long long r;
-    asm("mul.rn.ftz.f32x2 %0, %1, %2;" : "=l"(r) : "l"(f2bits(a)), "l"(f2bits(b)));
-    return f2from(r);
-}
-B2_DEV F2 sub2(const F2 &a, const F2 &b) {
-    unsigned long long r;
-    asm("sub.rn.ftz.f32x2 %0, %1, %2;" : "=l"(r) : "l"(f2bits(a)), "l"(f2bits(b)));
-    return f2from(r);
-}
+B2_DEV float fmaFtz(float a, float b, float c) { float r; asm("fma.rn.ftz.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c)); return r; }
+B2_DEV float mulFtz(float a, float b) { float r; asm("mul.rn.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
+B2_DEV float subFtz(float a, float b) { float r; asm("sub.rn.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
+B2_DEV F2 fma2(const F2 &a, const F2 &b, const F2 &c) { F2 r; r.x = fmaFtz(a.x, b.x, c.x); r.y = fmaFtz(a.y, b.y, c.y); return r; }
+B2_DEV F2 mul2(const F2 &a, const F2 &b) { F2 r; r.x = mulFtz(a.x, b.x); r.y = mulFtz(a.y, b.y); return r; }
+B2_DEV F2 sub2(const F2 &a, const F2 &b) { F2 r; r.x = subFtz(a.x, b.x); r.y = subFtz(a.y, b.y); return r; }
 B2_DEV F2 lo2(const float4 &v) { F2 r; r.x = v.x; r.y = v.y; return r; }
 B2_DEV F2 hi2(const float4 &v) { F2 r; r.x = v.z; r.y = v.w; return r; }
 B2_DEV F2 dup2(float v) { F2 r; r.x = v; r.y = v; return r; }

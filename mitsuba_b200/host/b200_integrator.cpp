@@ -271,5 +271,5 @@ private:
 };
 
 MTS_IMPLEMENT_CLASS_S(B200PathTracer, false, Integrator)
-MTS_EXPORT_PLUGIN(B200PathTracer, "B200 wavefront path tracer (libb2mts)");
+MTS_EXPORT_PLUGIN(B200PathTracer, "GPU wavefront path tracer (libb2mts)");
 MTS_NAMESPACE_END

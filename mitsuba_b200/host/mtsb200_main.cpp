@@ -9,7 +9,7 @@
 
 static void usage() {
     fprintf(stderr, "usage: mtsb200 [-o out.pfm] [-D key=value]... [-g gpu] [-q] scene.xml\n"
-                    "  renders <scene.xml> with the B200 wavefront `path` integrator (no CPU fallback)\n");
+                    "  renders <scene.xml> with the GPU wavefront `path` integrator (no CPU fallback)\n");
 }
 
 int main(int argc, char **argv) {

@@ -332,6 +332,19 @@ def spectrum_ref():
     print("spectrum_ref.npz:", len(out), "spectra")
 
 
+def conductor_ref():
+    """The conductor plugins' material presets as the reference derives them (InterpolatedSpectrum of data/ior/<name>.{eta,k}.spd +
+    Spectrum::fromContinuousSpectrum, through oracle/_ref/libpathref.so) for every material of the reference's data/ior."""
+    lib = C.CDLL(os.path.join(HERE, "..", "oracle", "_ref", "libpathref.so"))
+    f = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
+    names = sorted(n[:-len(".eta.spd")] for n in os.listdir(os.path.join(REF, "data", "ior")) if n.endswith(".eta.spd"))
+    eta, k = np.zeros((len(names), 3), np.float32), np.zeros((len(names), 3), np.float32)
+    for i, n in enumerate(names):
+        assert lib.pathref_conductor_preset(os.path.join(REF, "data").encode(), n.encode(), f(eta[i]), f(k[i])) == 0, n
+    np.savez_compressed(os.path.join(OUT, "conductor_ref.npz"), names=np.array(names), eta=eta, k=k)
+    print("conductor_ref.npz:", len(names), "materials")
+
+
 def path_ref_tex():
     """bitmap textures through the same assembled reference renderer (ref_pins.image_cases_tex): film + the reference's sampleToCamera."""
     sys.path.insert(0, HERE)
@@ -362,6 +375,9 @@ if __name__ == "__main__":
     if "--ext-only" in sys.argv:
         path_ref_ext()
         sys.exit(0)
+    if "--conductor-only" in sys.argv:
+        conductor_ref()
+        sys.exit(0)
     if "--texture-only" in sys.argv:
         half_ref()
         mipmap_ref()
@@ -371,6 +387,7 @@ if __name__ == "__main__":
     path_ref_env()
     path_ref_tex()
     spectrum_ref()
+    conductor_ref()
     render_ref()
     core_ref()
     bsdf_ref()

@@ -220,9 +220,9 @@ def test_material_ball_image_parity(b2ctx, name, sorted_shading):
     assert abs(sg["path_length_sum"] - so["pathLengthSum"]) <= 1e-3 * so["pathLengthSum"]
     if not sorted_shading:
         return
-    # Throughput build (the one bench.py times).  An ulp-level difference flips about 3e-5 of the paths of a rough dielectric (8e-6 rough
-    # conductor, 3e-6 diffuse: profiles/r02_parity_probe.json); a flipped path is an unrelated sample of a heavy-tailed estimator, so the
-    # image error behaves like 3.7 * sqrt(f / spp): 2.7e-3 at 32 spp whatever the kernel does, 4.5e-4 at 2048 spp.  The 1e-3 bar is
+    # Throughput build (the one bench.py times).  An ulp-level difference flips a fraction f of the paths (of order 1e-5; most for a rough
+    # dielectric, fewest for diffuse); a flipped path is an unrelated sample of a heavy-tailed estimator, so the image error behaves like
+    # 3.7 * sqrt(f / spp), which at low sample counts exceeds 1e-3 whatever the kernel does.  The 1e-3 bar is
     # therefore tested where it is resolvable, together with the diagnostic itself (fraction of pixels whose path lengths changed).
     # (flags 256 forces the throughput kernels: by default a `path` render of a scene with a transmissive BSDF is dispatched to the IEEE
     # kernels for exactly this reason, which the last assertion checks)

@@ -43,8 +43,8 @@ def test_device_images_of_thinlens_constant_emitter_and_instances_match_the_refe
         assert rel_l2(film[..., :3], ref[..., :3]) <= tol, (name, rel_l2(film[..., :3], ref[..., :3]))
         # the throughput build (FMA contraction, --use_fast_math, plane-form triangles; the build bench.py times) against the same
         # reference film: identical sample positions (weights), and every pixel within 1e-3 of the reference except the handful whose
-        # path was flipped by an ulp-level difference (one flipped path moves a pixel of these 4-16 spp fixtures by percents:
-        # measured 3e-5 of all paths for rough dielectrics, 3e-6 for diffuse scenes, profiles/r02_parity_probe.json)
+        # path was flipped by an ulp-level difference (one flipped path moves a pixel of these 4-16 spp fixtures by percents; rough
+        # dielectrics flip the most paths, diffuse scenes the fewest)
         fast = np.asarray(sc.render(rp, parity=False)[0]).reshape(ref.shape)
         assert np.allclose(fast[..., 4], ref[..., 4], rtol=1e-5, atol=1e-6), name
         rel = np.abs(fast[..., :3] - ref[..., :3]).max(-1) / np.maximum(np.abs(ref[..., :3]).max(-1), 1e-3 * ref[..., :3].max())

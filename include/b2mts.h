@@ -140,6 +140,9 @@ typedef struct b2_stats {
     uint64_t pool_size;                     /* in-flight paths of the last b2_render */
     uint64_t unoccluded_shadow_rays;        /* shadow rays that reached the emitter (their contribution was added) */
     uint64_t bvh_node_bytes;                /* size of one node of the tree the ray queries walk (80: 8-wide compressed, 64: binary) */
+    float accel_build_ms;                   /* acceleration-structure build of the last b2_scene_commit: host wall time of the builds, or
+                                               CUDA-event time of the device builds (box upload to leaf-order readback) */
+    int32_t accel_build_mode;               /* B2_ACCEL_BUILD_* that built it */
 } b2_stats;
 
 /* ---- lifetime -------------------------------------------------------------------------------- */
@@ -207,6 +210,27 @@ int b2_scene_add_instance(b2_scene *, int group_id, const float to_world[16], co
  * acceleration structure build (BVH; replaces GenericKDTree::buildInternal, gkdtree.h:958-1263),
  * emitter / triangle-area CDFs (scene.cpp:375-380, trimesh.cpp:388-403), upload to HBM. */
 int b2_scene_commit(b2_scene *);
+
+/* ---- acceleration-structure builder ------------------------------------------------------------------------------------------
+ * B2_ACCEL_BUILD_HOST: the multi-threaded binned-SAH builder on the CPU (the default).  B2_ACCEL_BUILD_DEVICE: the same builder on the
+ * GPU.  Both make byte-identical binary and 8-wide node arrays and the same leaf order, except that below a node split at the object
+ * median (all centroids equal, or the depth cap) each binary leaf holds the same triangles in an unspecified order.  The device build
+ * covers the world tree and every shapegroup's tree; scenes of at most 64 triangles and the top-level instance tree are built as before. */
+#define B2_ACCEL_BUILD_HOST 0
+#define B2_ACCEL_BUILD_DEVICE 1
+/* The builder b2_scene_commit uses for this scene; call before the commit.  B2_ERR_INVALID for a null scene, an unknown mode or a
+ * committed scene. */
+int b2_scene_set_accel_build(b2_scene *, int mode);
+/* The builder of scenes created on this context afterwards (b2_load_xml, which commits internally, uses it).  B2_ERR_INVALID for a null
+ * context or an unknown mode. */
+int b2_context_set_accel_build(b2_ctx *, int mode);
+/* The committed scene's acceleration arrays as they sit in device memory: which = B2_ACCEL_NODES (BVHNode, 64 bytes each),
+ * B2_ACCEL_NODES8 (BVH8Node, 80 bytes each; empty when the scene has no 8-wide tree) or B2_ACCEL_LEAF_PRIMS (uint32 prim ids in leaf
+ * order).  *bytes: in = capacity of `out`, out = size; out NULL = size query. */
+#define B2_ACCEL_NODES 0
+#define B2_ACCEL_NODES8 1
+#define B2_ACCEL_LEAF_PRIMS 2
+int b2_scene_get_accel(b2_scene *, int which, void *out, uint64_t *bytes);
 
 /* ---- the hot path: SamplingIntegrator::render + renderBlock + MIPathTracer::Li
  *      (src/librender/integrator.cpp:95-188, src/integrators/path/path.cpp:119-294) ------------- */

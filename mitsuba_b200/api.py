@@ -59,7 +59,8 @@ class b2_stats(C.Structure):
                                           "node_visits", "prim_tests", "iterations", "kernel_launches")] + \
                [(n, C.c_float) for n in ("ms_total", "ms_generate", "ms_extend", "ms_shade", "ms_occluded", "ms_film")] + \
                [(n, C.c_uint64) for n in ("n_triangles", "n_bvh_nodes", "n_generate", "n_extend", "n_shade", "n_occluded",
-                                          "bytes_uploaded", "pool_size", "unoccluded_shadow_rays", "bvh_node_bytes")]
+                                          "bytes_uploaded", "pool_size", "unoccluded_shadow_rays", "bvh_node_bytes")] + \
+               [("accel_build_ms", C.c_float), ("accel_build_mode", C.c_int32)]
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
@@ -69,7 +70,16 @@ EXPORTS = ["b2_context_create", "b2_context_destroy", "b2_last_error", "b2_scene
            "b2_scene_set_camera", "b2_scene_set_crop", "b2_scene_set_thinlens", "b2_scene_get_sample_to_camera", "b2_scene_film_size", "b2_scene_add_material", "b2_scene_add_area_emitter",
            "b2_scene_add_mesh", "b2_scene_add_shapegroup", "b2_scene_set_mesh_group", "b2_scene_add_instance", "b2_scene_add_constant_emitter", "b2_scene_add_envmap_emitter", "b2_envmap_probe", "b2_load_image", "b2_spectrum_to_rgb", "b2_scene_add_medium", "b2_scene_set_mesh_media", "b2_medium_probe", "b2_scene_add_texture", "b2_texture_eval", "b2_texture_partials", "b2_texture_level", "b2_mipmap_level", "b2_scene_commit", "b2_render", "b2_cancel", "b2_film_develop", "b2_get_stats", "b2_get_pixel_stats", "b2_get_path_traces", "b2_trace",
            "b2_trace_device", "b2_bsdf_eval", "b2_bsdf_sample", "b2_sample_emitter_direct", "b2_sampler_stream",
-           "b2_camera_rays", "b2_splat", "b2_get_triaccel", "b2_load_xml", "b2_version", "b2_device_count"]
+           "b2_camera_rays", "b2_splat", "b2_get_triaccel", "b2_load_xml", "b2_version", "b2_device_count",
+           "b2_scene_set_accel_build", "b2_context_set_accel_build", "b2_scene_get_accel"]
+
+ACCEL_BUILDS = {"host": 0, "device": 1}
+
+
+def _accel_mode(name):
+    if name not in ACCEL_BUILDS:
+        raise B2Error(f"accel_build must be one of {sorted(ACCEL_BUILDS)}, not {name!r}")
+    return ACCEL_BUILDS[name]
 
 
 def lib():
@@ -178,7 +188,15 @@ class Context:
             raise B2Error(self.err())
         return film
 
-    def load_xml(self, path, defines=()):
+    def set_accel_build(self, accel_build):
+        """Builder ("host" | "device") of the scenes created on this context from now on (b2_context_set_accel_build)."""
+        if self.L.b2_context_set_accel_build(self.h, C.c_int(_accel_mode(accel_build))):
+            raise B2Error(self.err())
+
+    def load_xml(self, path, defines=(), accel_build=None):
+        """accel_build: "host" | "device" sets the context's default builder first (it stays set for later scenes)."""
+        if accel_build is not None:
+            self.set_accel_build(accel_build)
         hs = C.c_void_p()
         p = b2_render_params()
         arr = (C.c_char_p * max(1, len(defines)))(*[d.encode() for d in defines])
@@ -197,10 +215,13 @@ class Context:
 class Scene:
     """Device scene built from a SceneDesc through the C-ABI."""
 
-    def __init__(self, ctx: Context, desc: SceneDesc):
+    def __init__(self, ctx: Context, desc: SceneDesc, accel_build=None):
+        """accel_build: "host" | "device" acceleration-structure builder; None = the context's default (host unless changed)."""
         self.ctx, self.L = ctx, ctx.L
         self.h = C.c_void_p()
         self._ck(self.L.b2_scene_create(ctx.h, C.byref(self.h)))
+        if accel_build is not None:
+            self._ck(self.L.b2_scene_set_accel_build(self.h, C.c_int(_accel_mode(accel_build))))
         cam = desc.camera
         self.W, self.H = cam.film_size()
         c2w = np.ascontiguousarray(cam.to_world, np.float32)
@@ -328,6 +349,18 @@ class Scene:
         """(H, W, n_samples) uint64 event traces of the last render(flags=64), one byte per bounce (include/b2mts.h)."""
         out = np.zeros((self.H, self.W, n_samples), np.uint64)
         self._ck(self.L.b2_get_path_traces(self.h, C.c_uint64(out.size), out.ctypes.data_as(C.POINTER(C.c_uint64))))
+        return out
+
+    def accel_arrays(self):
+        """The committed acceleration arrays as they sit in device memory (b2_scene_get_accel): binary nodes and 8-wide nodes as raw
+        bytes (64 / 80 bytes per node), leaf-ordered prim ids as uint32."""
+        out = {}
+        for key, which in (("nodes", 0), ("nodes8", 1), ("leaf_prims", 2)):
+            n = C.c_uint64()
+            self._ck(self.L.b2_scene_get_accel(self.h, C.c_int(which), None, C.byref(n)))
+            buf = np.zeros(n.value, np.uint8)
+            self._ck(self.L.b2_scene_get_accel(self.h, C.c_int(which), buf.ctypes.data_as(C.c_void_p), C.byref(n)))
+            out[key] = buf.tobytes() if key != "leaf_prims" else buf.view(np.uint32)
         return out
 
     def triaccel(self):

@@ -4,6 +4,7 @@
 #include "b2_types.h"
 #include "b2_launch.h"
 #include "bvh_builder.h"
+#include "bvh_device.h"
 #include "../host/mipmap.h"
 
 #include <cuda_runtime.h>
@@ -43,6 +44,7 @@ struct b2_ctx {
     uint64_t *dVdc = nullptr, *dInv = nullptr;
     std::vector<uint64_t> hVdc, hInv; // host copies: per-render look_up nibble tables are derived from them
     bool tablesLoaded = false;
+    int accelBuild = B2_ACCEL_BUILD_HOST; // builder of the scenes created from now on (b2_context_set_accel_build)
 };
 
 static int fail(b2_ctx *ctx, int code, const std::string &msg) {
@@ -173,6 +175,7 @@ struct b2_scene {
     b2_stats stats{};
     uint32_t nPrims = 0;
     int bvhDepth = 0;
+    int accelBuild = B2_ACCEL_BUILD_HOST;
 };
 
 // The kernel build that runs a render or a component call: the IEEE build (b2::parity, -fmad=false) or the throughput build
@@ -298,6 +301,7 @@ extern "C" int b2_scene_create(b2_ctx *ctx, b2_scene **out) {
     if (!ctx || !out) return fail(ctx, B2_ERR_INVALID, "b2_scene_create: null argument");
     b2_scene *s = new b2_scene();
     s->ctx = ctx;
+    s->accelBuild = ctx->accelBuild;
     *out = s;
     return B2_OK;
 }
@@ -691,6 +695,28 @@ struct CommitClock {
         last = now;
     }
 };
+static bool validAccelBuild(int mode) { return mode == B2_ACCEL_BUILD_HOST || mode == B2_ACCEL_BUILD_DEVICE; }
+extern "C" int b2_scene_set_accel_build(b2_scene *s, int mode) {
+    if (!s) return fail(nullptr, B2_ERR_INVALID, "b2_scene_set_accel_build: null scene");
+    if (!validAccelBuild(mode))
+        return fail(s->ctx, B2_ERR_INVALID, "b2_scene_set_accel_build: unknown mode " + std::to_string(mode) + " (B2_ACCEL_BUILD_HOST = 0, B2_ACCEL_BUILD_DEVICE = 1)");
+    if (s->committed) return fail(s->ctx, B2_ERR_INVALID, "b2_scene_set_accel_build: the scene is already committed; choose the builder before b2_scene_commit");
+    s->accelBuild = mode;
+    return B2_OK;
+}
+extern "C" int b2_context_set_accel_build(b2_ctx *ctx, int mode) {
+    if (!ctx) return fail(nullptr, B2_ERR_INVALID, "b2_context_set_accel_build: null context");
+    if (!validAccelBuild(mode))
+        return fail(ctx, B2_ERR_INVALID, "b2_context_set_accel_build: unknown mode " + std::to_string(mode) + " (B2_ACCEL_BUILD_HOST = 0, B2_ACCEL_BUILD_DEVICE = 1)");
+    ctx->accelBuild = mode;
+    return B2_OK;
+}
+// a binary-tree reference moved into merged node / leaf arrays
+static int32_t shiftRef(int32_t r, uint32_t nodeBase, uint32_t leafBase) {
+    if (r >= 0) return r + (int32_t) nodeBase;
+    const uint32_t bits = ~(uint32_t) r;
+    return (int32_t) ~(((bits & 0x0FFFFFFFu) + leafBase) | (bits & 0xF0000000u));
+}
 extern "C" int b2_scene_commit(b2_scene *s) {
     if (!s) return fail(nullptr, B2_ERR_INVALID, "b2_scene_commit: null scene");
     b2_ctx *ctx = s->ctx;
@@ -817,6 +843,26 @@ extern "C" int b2_scene_commit(b2_scene *s) {
     // ---- BVH ----
     BVHResult bvh;
     int threads = usableThreads();
+    // B2_ACCEL_BUILD_DEVICE: the world and shapegroup trees are built on the device and their nodes stay there (devWorld, devGroups);
+    // bvh then carries the leaf order, root, depths and the host-built top-level nodes only
+    const bool devBuild = s->accelBuild == B2_ACCEL_BUILD_DEVICE;
+    std::unique_ptr<DeviceBVHResult> devWorld;
+    struct DevGroup { std::unique_ptr<DeviceBVHResult> r; uint32_t nodeBase, leafBase; };
+    std::vector<DevGroup> devGroups;
+    size_t devNodes = 0, devNodes8 = 0, devUploadBytes = 0; // device-resident binary / wide nodes, box + id bytes uploaded for the builds
+    double accelMs = 0;
+    auto deviceBuild = [&](const std::vector<PrimBox> &bx, const std::vector<uint32_t> &bi, int maxDepth, bool wide, DeviceBVHResult &r) -> int {
+        const std::string e = buildBVHDevice(bx, bi, 4, maxDepth, wide, ctx->stream, r);
+        if (!e.empty()) return fail(ctx, B2_ERR_CUDA, e);
+        accelMs += r.ms;
+        devUploadBytes += bx.size() * (sizeof(PrimBox) + sizeof(uint32_t));
+        return B2_OK;
+    };
+    auto hostBuild = [&](const std::vector<PrimBox> &bx, const std::vector<uint32_t> &bi, int maxDepth, int nThreads, BVHResult &r, bool wide) {
+        const auto t0 = std::chrono::steady_clock::now();
+        buildBVH(bx, bi, 4, maxDepth, nThreads, r, wide);
+        accelMs += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    };
     // Tiny scenes skip the tree: the whole triangle list is one leaf, staged in shared memory and tested by all lanes
     // in lockstep (no divergence).  Break-even against the BVH2 walk measured on the Cornell scene, see DESIGN.md.
     const uint32_t flatLimit = 64;
@@ -826,10 +872,17 @@ extern "C" int b2_scene_commit(b2_scene *s) {
         bvh.rootRef = -1; // ~0: leaf starting at triangle 0
         bvh.depth = 1;
         rootCount = (uint32_t) ids.size();
+    } else if (devBuild) {
+        devWorld.reset(new DeviceBVHResult());
+        if (int rc = deviceBuild(boxes, ids, instanced ? 19 : B2_STACK_DEPTH - 2, !instanced, *devWorld)) return rc;
+        bvh.leafPrims.swap(devWorld->leafPrims);
+        bvh.rootRef = devWorld->rootRef; bvh.depth = devWorld->depth; bvh.depth8 = devWorld->depth8;
+        devNodes = devWorld->nNodes;
+        devNodes8 = bvh.depth8 > B2_STACK8_DEPTH - 1 ? 0 : devWorld->nNodes8; // as below
     } else {
         // non-instanced scenes also get the 8-wide compressed tree over the same leaves: that is what the ray-query kernels walk (the binary
         // tree stays for volpath's inline queries)
-        buildBVH(boxes, ids, 4, instanced ? 19 : B2_STACK_DEPTH - 2, threads > 0 ? threads : 1, bvh, !instanced);
+        hostBuild(boxes, ids, instanced ? 19 : B2_STACK_DEPTH - 2, threads > 0 ? threads : 1, bvh, !instanced);
         if (bvh.depth8 > B2_STACK8_DEPTH - 1) bvh.nodes8.clear(); // deeper than the wide traversal's stack: binary tree only
     }
     clk.mark("BVH (world)");
@@ -843,20 +896,25 @@ extern "C" int b2_scene_commit(b2_scene *s) {
         std::vector<GroupInfo> gi((size_t) s->nGroups);
         auto appendTree = [&](BVHResult &g) -> int { // returns the root reference inside the merged arrays
             const uint32_t nodeBase = (uint32_t) bvh.nodes.size(), leafBase = (uint32_t) bvh.leafPrims.size();
-            auto fix = [&](int32_t r) -> int32_t {
-                if (r >= 0) return r + (int32_t) nodeBase;
-                const uint32_t bits = ~(uint32_t) r;
-                return (int32_t) ~(((bits & 0x0FFFFFFFu) + leafBase) | (bits & 0xF0000000u));
-            };
-            for (auto nd : g.nodes) { nd.left = fix(nd.left); nd.right = fix(nd.right); bvh.nodes.push_back(nd); }
+            for (auto nd : g.nodes) { nd.left = shiftRef(nd.left, nodeBase, leafBase); nd.right = shiftRef(nd.right, nodeBase, leafBase); bvh.nodes.push_back(nd); }
             bvh.leafPrims.insert(bvh.leafPrims.end(), g.leafPrims.begin(), g.leafPrims.end());
-            return fix(g.rootRef);
+            return shiftRef(g.rootRef, nodeBase, leafBase);
         };
         for (int g = 0; g < s->nGroups; ++g) {
             if (bIds[g + 1].empty()) continue;
             BVHResult r;
-            buildBVH(bBoxes[g + 1], bIds[g + 1], 4, 19, threads > 0 ? threads : 1, r);
-            gi[g].rootRef = appendTree(r);
+            if (devBuild) { // the nodes are merged on the device at upload
+                DevGroup dg{std::unique_ptr<DeviceBVHResult>(new DeviceBVHResult()), (uint32_t) devNodes, (uint32_t) bvh.leafPrims.size()};
+                if (int rc = deviceBuild(bBoxes[g + 1], bIds[g + 1], 19, false, *dg.r)) return rc;
+                gi[g].rootRef = shiftRef(dg.r->rootRef, dg.nodeBase, dg.leafBase);
+                bvh.leafPrims.insert(bvh.leafPrims.end(), dg.r->leafPrims.begin(), dg.r->leafPrims.end());
+                r.depth = dg.r->depth;
+                devNodes += dg.r->nNodes;
+                devGroups.push_back(std::move(dg));
+            } else {
+                hostBuild(bBoxes[g + 1], bIds[g + 1], 19, threads > 0 ? threads : 1, r, false);
+                gi[g].rootRef = appendTree(r);
+            }
             gi[g].empty = false;
             float l[3] = {INFINITY, INFINITY, INFINITY}, h[3] = {-INFINITY, -INFINITY, -INFINITY};
             for (auto &b : bBoxes[g + 1]) for (int a = 0; a < 3; ++a) { l[a] = std::min(l[a], b.lo[a]); h[a] = std::max(h[a], b.hi[a]); }
@@ -897,7 +955,7 @@ extern "C" int b2_scene_commit(b2_scene *s) {
         buildBVH(itemBoxes, itemIds, 4, 9, 1, top);
         if (top.depth > 10) return fail(ctx, B2_ERR_INVALID, "instance hierarchy too deep for the traversal stack");
         // top-level leaves reference items, not triangles: keep their refs apart from the triangle leaf array
-        const uint32_t nodeBase = (uint32_t) bvh.nodes.size();
+        const uint32_t nodeBase = (uint32_t) (devNodes + bvh.nodes.size());
         std::vector<uint32_t> order = top.leafPrims; // item order of the top-level leaves
         std::vector<DInstance> sorted(items.size());
         for (size_t k = 0; k < order.size(); ++k) sorted[k] = items[order[k]];
@@ -911,6 +969,8 @@ extern "C" int b2_scene_commit(b2_scene *s) {
         lo[0] = topLo[0]; lo[1] = topLo[1]; lo[2] = topLo[2]; hi[0] = topHi[0]; hi[1] = topHi[1]; hi[2] = topHi[2];
     }
     s->bvhDepth = bvh.depth;
+    // node counts of the arrays the traversal walks (the device build keeps the world / shapegroup nodes on the device)
+    const size_t nNodes = devNodes + bvh.nodes.size(), nNodes8 = devBuild ? devNodes8 : bvh.nodes8.size();
     std::vector<float4> leafTri(3 * bvh.leafPrims.size()), leafPlane(3 * bvh.leafPrims.size());
     // plane form of triangle (a, b, c), evaluated in double: N = e1 x e2, U = (e2 x N)/|N|^2, V = (N x e1)/|N|^2;
     // u(p) = U.p + du and v(p) = V.p + dv are the barycentrics of b and c
@@ -1022,7 +1082,7 @@ extern "C" int b2_scene_commit(b2_scene *s) {
     }
     if (getenv("B2_VERBOSE"))
         fprintf(stderr, "[b2mts] commit: %zu triangles, flat leaf %u (two-wide steps: parallelograms %u, coplanar pairs %u, singles %u), bvh nodes %zu depth %d\n", nPrims, rootCount,
-                flatP, flatC, flatS, bvh.nodes.size(), bvh.depth);
+                flatP, flatC, flatS, nNodes, bvh.depth);
     clk.mark("leaf records");
     // ---- materials ----
     std::vector<DMaterial> dm(s->materials.size());
@@ -1229,8 +1289,26 @@ extern "C" int b2_scene_commit(b2_scene *s) {
     CK(ctx, s->dFlatIdx.upload(flatIdx));
     CK(ctx, s->dVerts.upload(verts));
     CK(ctx, s->dNorms.upload(norms));
-    CK(ctx, s->dNodes.upload(bvh.nodes));
-    CK(ctx, s->dNodes8.upload(bvh.nodes8));
+    if (devBuild) {
+        if (!instanced && devWorld) { // the world tree's arrays become the scene's
+            s->dNodes.release(); s->dNodes.p = devWorld->nodes; s->dNodes.n = devWorld->nNodes; devWorld->nodes = nullptr;
+        } else {
+            CK(ctx, s->dNodes.alloc(nNodes));
+            if (devWorld && devWorld->nNodes)
+                CK(ctx, cudaMemcpyAsync(s->dNodes.p, devWorld->nodes, devWorld->nNodes * sizeof(BVHNode), cudaMemcpyDeviceToDevice, ctx->stream));
+            for (const DevGroup &g : devGroups) CK(ctx, appendTreeDevice(s->dNodes.p + g.nodeBase, g.r->nodes, g.r->nNodes, g.nodeBase, g.leafBase, ctx->stream));
+            if (!bvh.nodes.empty()) // the top-level instance tree, built on the host
+                CK(ctx, cudaMemcpyAsync(s->dNodes.p + devNodes, bvh.nodes.data(), bvh.nodes.size() * sizeof(BVHNode), cudaMemcpyHostToDevice, ctx->stream));
+            CK(ctx, cudaStreamSynchronize(ctx->stream));
+        }
+        s->dNodes8.release();
+        if (nNodes8) { s->dNodes8.p = devWorld->nodes8; s->dNodes8.n = nNodes8; devWorld->nodes8 = nullptr; }
+        devWorld.reset();
+        devGroups.clear();
+    } else {
+        CK(ctx, s->dNodes.upload(bvh.nodes));
+        CK(ctx, s->dNodes8.upload(bvh.nodes8));
+    }
     CK(ctx, s->dMaterials.upload(dm));
     CK(ctx, s->dEmitters.upload(de));
     CK(ctx, s->dEmitterCdf.upload(emCdf));
@@ -1262,8 +1340,8 @@ extern "C" int b2_scene_commit(b2_scene *s) {
     }
     ds.items = s->dInstances.p; ds.nItems = (uint32_t) items.size(); ds.tlasRoot = tlasRoot;
     ds.media = s->dMedia.p; ds.primMedia = anyMedia ? s->dPrimMedia.p : nullptr; ds.nMedia = (uint32_t) dmed.size();
-    ds.nodes8 = bvh.nodes8.empty() ? nullptr : s->dNodes8.p; ds.nNodes8 = (uint32_t) bvh.nodes8.size();
-    ds.nodes = s->dNodes.p; ds.nNodes = (uint32_t) bvh.nodes.size(); ds.rootRef = bvh.rootRef; ds.rootCount = rootCount;
+    ds.nodes8 = nNodes8 ? s->dNodes8.p : nullptr; ds.nNodes8 = (uint32_t) nNodes8;
+    ds.nodes = s->dNodes.p; ds.nNodes = (uint32_t) nNodes; ds.rootRef = bvh.rootRef; ds.rootCount = rootCount;
     ds.flatRec = s->dFlatRec.p; ds.flatIdx = (const uint2 *) s->dFlatIdx.p; ds.flatP = flatP; ds.flatC = flatC; ds.flatS = flatS;
     ds.flatBytes = (uint32_t) (flatRec.size() * 16);
     // gkdtree.h:1213-1220: enlarged scene box (the max side uses the already-moved min, as in the reference)
@@ -1319,12 +1397,34 @@ extern "C" int b2_scene_commit(b2_scene *s) {
     CK(ctx, s->dCounters.alloc(CTR_COUNT));
     memset(&s->stats, 0, sizeof(s->stats));
     s->stats.n_triangles = nPrims;
-    s->stats.n_bvh_nodes = bvh.nodes8.empty() ? bvh.nodes.size() : bvh.nodes8.size();
-    s->stats.bvh_node_bytes = bvh.nodes8.empty() ? sizeof(BVHNode) : sizeof(BVH8Node);
-    s->stats.bytes_uploaded = leafTri.size() * 16 + leafPlane.size() * 16 + bvh.leafPrims.size() * 4 + verts.size() * 16 + norms.size() * 16 + bvh.nodes.size() * sizeof(BVHNode) +
+    s->stats.n_bvh_nodes = nNodes8 ? nNodes8 : nNodes;
+    s->stats.bvh_node_bytes = nNodes8 ? sizeof(BVH8Node) : sizeof(BVHNode);
+    s->stats.accel_build_ms = (float) accelMs;
+    s->stats.accel_build_mode = s->accelBuild;
+    s->stats.bytes_uploaded = leafTri.size() * 16 + leafPlane.size() * 16 + bvh.leafPrims.size() * 4 + verts.size() * 16 + norms.size() * 16 + bvh.nodes.size() * sizeof(BVHNode) + devUploadBytes +
                               dm.size() * sizeof(DMaterial) + de.size() * sizeof(DEmitter) + (emCdf.size() + triCdf.size()) * 4;
     clk.mark("upload");
     s->committed = true;
+    return B2_OK;
+}
+
+extern "C" int b2_scene_get_accel(b2_scene *s, int which, void *out, uint64_t *bytes) {
+    if (!s || !bytes) return fail(s ? s->ctx : nullptr, B2_ERR_INVALID, "b2_scene_get_accel: null argument");
+    if (!s->committed) return fail(s->ctx, B2_ERR_INVALID, "b2_scene_get_accel: scene not committed");
+    const DScene &ds = s->ds;
+    const void *src = nullptr;
+    uint64_t size = 0;
+    switch (which) {
+    case B2_ACCEL_NODES: src = ds.nodes; size = (uint64_t) ds.nNodes * sizeof(BVHNode); break;
+    case B2_ACCEL_NODES8: src = ds.nodes8; size = ds.nodes8 ? (uint64_t) ds.nNodes8 * sizeof(BVH8Node) : 0; break;
+    case B2_ACCEL_LEAF_PRIMS: src = ds.leafPrim; size = (uint64_t) ds.nLeafTris * sizeof(uint32_t); break;
+    default: return fail(s->ctx, B2_ERR_INVALID, "b2_scene_get_accel: unknown array " + std::to_string(which));
+    }
+    if (!out) { *bytes = size; return B2_OK; }
+    if (*bytes < size) return fail(s->ctx, B2_ERR_INVALID, "b2_scene_get_accel: buffer too small");
+    CK(s->ctx, cudaSetDevice(s->ctx->device));
+    if (size) CK(s->ctx, cudaMemcpy(out, src, size, cudaMemcpyDeviceToHost));
+    *bytes = size;
     return B2_OK;
 }
 

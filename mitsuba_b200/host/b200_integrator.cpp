@@ -63,6 +63,11 @@ public:
         m_hideEmitters = props.getBoolean("hideEmitters", false);
         m_device = props.getInteger("device", 0);
         m_parity = props.getBoolean("parity", false);
+        /* acceleration-structure builder of b2_scene_commit: "host" (multi-threaded CPU build) or "device" (the same tree built on the GPU) */
+        const std::string accelBuild = props.getString("accelBuild", "host");
+        if (accelBuild == "host") m_accelBuild = B2_ACCEL_BUILD_HOST;
+        else if (accelBuild == "device") m_accelBuild = B2_ACCEL_BUILD_DEVICE;
+        else Log(EError, "'accelBuild' must be \"host\" or \"device\", not \"%s\"", accelBuild.c_str());
         if (m_rrDepth <= 0) Log(EError, "'rrDepth' must be set to a value greater than zero!");
         if (m_maxDepth <= 0 && m_maxDepth != -1) Log(EError, "'maxDepth' must be set to -1 (infinite) or a value greater than zero!");
     }
@@ -70,12 +75,14 @@ public:
         m_rrDepth = stream->readInt(); m_maxDepth = stream->readInt();
         m_strictNormals = stream->readBool(); m_hideEmitters = stream->readBool();
         m_device = stream->readInt(); m_parity = stream->readBool();
+        m_accelBuild = stream->readInt();
     }
     void serialize(Stream *stream, InstanceManager *manager) const {
         Integrator::serialize(stream, manager);
         stream->writeInt(m_rrDepth); stream->writeInt(m_maxDepth);
         stream->writeBool(m_strictNormals); stream->writeBool(m_hideEmitters);
         stream->writeInt(m_device); stream->writeBool(m_parity);
+        stream->writeInt(m_accelBuild);
     }
 
     /* BSDF plugin -> b2_material_desc from its construction Properties: the same host-side preprocessing the plugin constructors do
@@ -152,6 +159,7 @@ public:
         b2_scene *sc = NULL;
         if (b2_context_create(m_device, &ctx)) Log(EError, "%s", b2_last_error(NULL)); /* Log(EError) throws */
         if (b2_scene_create(ctx, &sc)) Log(EError, "%s", b2_last_error(ctx));
+        if (b2_scene_set_accel_build(sc, m_accelBuild)) Log(EError, "%s", b2_last_error(ctx));
         m_handle = sc;
         /* ---- sensor + film: src/sensors/{perspective,thinlens}.cpp, film.cpp:36-47 ---- */
         const Sensor *sensor = scene->getSensor();
@@ -267,6 +275,7 @@ public:
 private:
     int m_rrDepth, m_maxDepth, m_device;
     bool m_strictNormals, m_hideEmitters, m_parity;
+    int m_accelBuild;
     void *m_handle;
 };
 

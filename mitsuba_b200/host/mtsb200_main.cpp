@@ -8,8 +8,9 @@
 #include <vector>
 
 static void usage() {
-    fprintf(stderr, "usage: mtsb200 [-o out.pfm] [-D key=value]... [-g gpu] [-q] scene.xml\n"
-                    "  renders <scene.xml> with the GPU wavefront `path` integrator (no CPU fallback)\n");
+    fprintf(stderr, "usage: mtsb200 [-o out.pfm] [-D key=value]... [-g gpu] [-q] [--accel-build host|device] scene.xml\n"
+                    "  renders <scene.xml> with the GPU wavefront `path` integrator (no CPU fallback)\n"
+                    "  --accel-build  builder of the acceleration structure: host (multi-threaded CPU, the default) or device (GPU)\n");
 }
 
 int main(int argc, char **argv) {
@@ -17,12 +18,19 @@ int main(int argc, char **argv) {
     std::vector<const char *> defs;
     int gpu = 0;
     bool quiet = false;
+    int accelBuild = B2_ACCEL_BUILD_HOST;
     for (int i = 1; i < argc; ++i) {
         if (!strcmp(argv[i], "-o") && i + 1 < argc) out = argv[++i];
         else if (!strcmp(argv[i], "-D") && i + 1 < argc) defs.push_back(argv[++i]);
         else if (!strncmp(argv[i], "-D", 2) && argv[i][2]) defs.push_back(argv[i] + 2);
         else if (!strcmp(argv[i], "-g") && i + 1 < argc) gpu = atoi(argv[++i]);
         else if (!strcmp(argv[i], "-q")) quiet = true;
+        else if (!strcmp(argv[i], "--accel-build") && i + 1 < argc) {
+            const char *m = argv[++i];
+            if (!strcmp(m, "host")) accelBuild = B2_ACCEL_BUILD_HOST;
+            else if (!strcmp(m, "device")) accelBuild = B2_ACCEL_BUILD_DEVICE;
+            else { fprintf(stderr, "--accel-build must be host or device, not %s\n", m); usage(); return 2; }
+        }
         else if (!strcmp(argv[i], "-h")) { usage(); return 0; }
         else if (argv[i][0] == '-') { fprintf(stderr, "unknown option %s\n", argv[i]); usage(); return 2; }
         else scene = argv[i];
@@ -31,6 +39,7 @@ int main(int argc, char **argv) {
     if (out.empty()) { out = scene; size_t k = out.rfind('.'); if (k != std::string::npos) out.resize(k); out += ".pfm"; } // mitsuba.cpp:381-386
     b2_ctx *ctx = nullptr;
     if (b2_context_create(gpu, &ctx)) { fprintf(stderr, "error: %s\n", b2_last_error(nullptr)); return 1; }
+    if (b2_context_set_accel_build(ctx, accelBuild)) { fprintf(stderr, "error: %s\n", b2_last_error(ctx)); return 1; }
     b2_scene *sc = nullptr;
     b2_render_params rp;
     if (b2_load_xml(ctx, scene.c_str(), defs.data(), (int) defs.size(), &sc, &rp)) { fprintf(stderr, "error: %s\n", b2_last_error(ctx)); return 1; }

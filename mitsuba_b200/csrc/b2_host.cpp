@@ -1684,12 +1684,18 @@ extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
         ++evUsed;
     };
     int launchesPerIter = 0;
-    // one iteration = generate (+publish) -> extend -> shade (per material class) -> occluded
+    // one iteration = generate (+publish) -> extend -> shade (per material class) -> occluded; flat scenes shaded by one launch:
+    // generate (+publish) -> bounce
     auto enqueueIteration = [&]() {
         launchesPerIter = 0;
         tick(0); K.generate(cfg, s->ds, s->pool, r, filt, st); tick(-1);
         if (volpath) { // volpath: every ray of an iteration is cast inline by k_volstep_lockstep
             tick(2); K.volstep(cfg, s->ds, s->pool, r, st); tick(-1);
+            launchesPerIter = 3;
+            return;
+        }
+        if (s->ds.rootCount && !sorted) { // shared-memory resident scene, one shading instance: extend + shade + occluded in one launch
+            tick(2); K.bounce_flat(cfg, s->ds, s->pool, r, nClasses == 1 ? onlyClass : -1, st); tick(-1);
             launchesPerIter = 3;
             return;
         }

@@ -15,9 +15,10 @@ struct LaunchCfg {
     int gridShade[5] = {0, 0, 0, 0, 0};
     int gridShadeTex = 0; // k_shade<-1, TEX = true> (textured scenes)
     int gridShadeTexCls[4] = {0, 0, 0, 0}; // k_shade<c, TEX = true>: class-sorted dispatch of textured / environment-mapped scenes
-    // flat-leaf variants (shared-memory resident scenes): k_extend_flat / k_occluded_flat
+    // flat-leaf variants (shared-memory resident scenes): k_extend_flat / k_occluded_flat (class-sorted), k_bounce_flat[TEX][class]
     size_t flatSmem = 0;
-    int gridExtendFlat = 0, gridExtendFlatSort = 0, gridOccludedFlat = 0;
+    int gridExtendFlatSort = 0, gridOccludedFlat = 0;
+    int gridBounceFlat[2][5] = {{0, 0, 0, 0, 0}, {0, 0, 0, 0, 0}};
 };
 
 struct KernelSet {
@@ -26,6 +27,8 @@ struct KernelSet {
     void (*extend)(const LaunchCfg &, const DScene &, const DPool &, const DRender &, bool sort, cudaStream_t);
     void (*shade)(const LaunchCfg &, const DScene &, const DPool &, const DRender &, int cls, bool queued, cudaStream_t);
     void (*occluded)(const LaunchCfg &, const DScene &, const DPool &, const DRender &, cudaStream_t);
+    // flat scenes shaded by one launch: extend + shade + occluded in one kernel, cls as for shade (unqueued)
+    void (*bounce_flat)(const LaunchCfg &, const DScene &, const DPool &, const DRender &, int cls, cudaStream_t);
     void (*volstep)(const LaunchCfg &, const DScene &, const DPool &, const DRender &, cudaStream_t);
     void (*medium_probe)(const LaunchCfg &, const DScene &, int medium, int what, uint64_t n, const float *in, uint64_t seed, float *out,
                          cudaStream_t);

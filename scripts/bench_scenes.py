@@ -63,6 +63,15 @@ if "cornell" in which:
     render_rate("cornell_box", d, RenderParams(spp=64, rfilter="box"))
     render_rate("cornell_box", d, RenderParams(spp=64, rfilter="box", sampler="independent"))
     trace_bench("cornell_box", sc, d)
+if "cornell_mixed" in which:
+    # two BSDF classes in one flat leaf (the short block a GGX rough conductor): the class-sorted dispatch (k_extend_flat, one k_shade per
+    # class, k_occluded_flat) against k_bounce_flat with the generic shading instance (flags bit1)
+    d = cornell_box(1024, 1024)
+    for m in d.meshes:
+        if m.name == "short":
+            m.bsdf = Bsdf("roughconductor", distribution="ggx", alpha_u=0.2, alpha_v=0.2, **CU)
+    sc = render_rate("cornell_mixed/sorted", d, RenderParams(spp=64, rfilter="box"))
+    render_rate("cornell_mixed/bounce", d, RenderParams(spp=64, rfilter="box"), flags=4 | 2)
 if "ball" in which:
     for nm, b in (("roughconductor_ggx", Bsdf("roughconductor", distribution="ggx", alpha_u=0.1, alpha_v=0.1, **CU)),
                   ("roughdielectric_ggx", Bsdf("roughdielectric", distribution="ggx", alpha_u=0.1, alpha_v=0.1, int_ior="bk7", ext_ior="air")),

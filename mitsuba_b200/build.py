@@ -28,6 +28,7 @@ UNITS = [
     # parity tests hold it to the same 1e-3 relative-L2 tolerance as the parity build
     (os.path.join(CSRC, "kernels_fast.cu"), ["--use_fast_math"]),
     (os.path.join(CSRC, "b2_host.cpp"), ["-x", "cu"]),
+    (os.path.join(CSRC, "b2_commit.cpp"), ["-x", "cu"]),
     (os.path.join(CSRC, "bvh_builder.cpp"), []),
     # device BVH build: byte-identical to bvh_builder.cpp, so IEEE arithmetic without contraction (division and sqrt stay IEEE)
     (os.path.join(CSRC, "bvh_device.cu"), ["-fmad=false"]),
@@ -36,7 +37,7 @@ UNITS = [
     (os.path.join(HOST, "spectrum.cpp"), []),
 ]
 HEADERS = [os.path.join(CSRC, f) for f in ("b2_math.cuh", "b2_types.h", "b2_sampler.cuh", "b2_bsdf.cuh", "b2_trace.cuh",
-                                           "b2_kernels.inl", "b2_launch.h", "bvh_builder.h", "bvh_device.h", "b2_medium.cuh", "b2_texture.cuh", "b2_envmap.cuh")] + \
+                                           "b2_kernels.inl", "b2_launch.h", "b2_host.h", "bvh_builder.h", "bvh_device.h", "b2_medium.cuh", "b2_texture.cuh", "b2_envmap.cuh")] + \
           [os.path.join(HOST, "mipmap.h"), os.path.join(HOST, "spectrum.h")] + \
           [os.path.join(HERE, "..", "include", "b2mts.h")]
 

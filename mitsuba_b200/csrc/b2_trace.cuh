@@ -34,6 +34,20 @@ struct HitRec {
     uint32_t leaf;   // leaf-ordered index of the triangle (into triAccel / triPlane); valid when prim is
 };
 
+// (t, u, v, prim) of a miss (leaf is not set)
+B2_DEV HitRec missHit() {
+    HitRec h;
+    h.t = B2_INF; h.u = 0; h.v = 0; h.prim = 0xFFFFFFFFu;
+    return h;
+}
+// the pool's hit record (DPool::hit): (t, u, v, prim)
+B2_DEV float4 packHit(const HitRec &h) { return make_float4(h.t, h.u, h.v, __uint_as_float(h.prim)); }
+B2_DEV HitRec unpackHit(const float4 &r) {
+    HitRec h;
+    h.t = r.x; h.u = r.y; h.v = r.z; h.prim = __float_as_uint(r.w);
+    return h;
+}
+
 // triaccel.h:96-158
 B2_DEV bool triAccelIntersect(const float4 &q0, const float4 &q1, const float4 &q2, const V3 &o, const V3 &d, float mint,
                               float maxt, float &u, float &v, float &t) {
@@ -93,14 +107,10 @@ B2_DEV bool aabbRayIntersect(const float *bmin, const float *bmax, const V3 &o, 
     return true;
 }
 
-B2_DEV bool sceneBoxIntersect(const DScene &sc, const V3 &o, const V3 &d, const V3 &dRcp, float &nearT, float &farT) {
-    return aabbRayIntersect(sc.aabbMin, sc.aabbMax, o, d, dRcp, nearT, farT);
-}
-
 // skdtree.cpp:124-133 (closest) / :211-218 (occlusion): clip to the scene box and apply the adaptive epsilon
-template <bool SHADOW> B2_DEV bool clipRay(const DScene &sc, const V3 &o, const V3 &d, const V3 &dRcp, float rayMint, float rayMaxt,
-                                            float &mint, float &maxt) {
-    if (!sceneBoxIntersect(sc, o, d, dRcp, mint, maxt)) return false;
+template <bool SHADOW> B2_DEV bool clipRay(const DScene &sc, const V3 &o, const V3 &d, float rayMint, float rayMaxt, float &mint, float &maxt) {
+    const V3 dRcp(1.0f / d.x, 1.0f / d.y, 1.0f / d.z); // ray.h:83-84
+    if (!aabbRayIntersect(sc.aabbMin, sc.aabbMax, o, d, dRcp, mint, maxt)) return false;
     float rayMinT = rayMint;
     if (rayMinT == B2_EPSILON) {
         float m = fmaxf(fmaxf(fabsf(o.x), fabsf(o.y)), fabsf(o.z));
@@ -339,6 +349,18 @@ template <bool SHADOW, bool COUNT> B2_DEV bool traverse(const DScene &sc, const 
     return found;
 }
 
+// One ray traced inline by the calling thread: clip to the scene box with the epsilon of a closest (CLIP_SHADOW = false) or an
+// occlusion query, then a closest or any-hit (SHADOW) walk of the flat leaf (FLAT) or of whichever of the flat leaf and the binary
+// tree the scene has.  Returns whether something was hit; otherwise `hit` is the miss record.
+template <bool SHADOW, bool CLIP_SHADOW, bool FLAT>
+B2_DEV bool traceRay(const DScene &sc, const TraceMem &tm, const V3 &o, const V3 &d, float rayMint, float rayMaxt, HitRec &hit) {
+    hit = missHit();
+    float mint, maxt;
+    uint32_t nv = 0, pt = 0;
+    if (!clipRay<CLIP_SHADOW>(sc, o, d, rayMint, rayMaxt, mint, maxt)) return false;
+    return FLAT ? traverseFlat<SHADOW, false>(sc, tm, o, d, mint, maxt, hit, pt) : traverse<SHADOW, false>(sc, tm, o, d, mint, maxt, hit, nv, pt);
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // Instanced scenes (src/shapes/{shapegroup,instance}.cpp): a top-level BVH over items (the world triangles, each `instance`),
 // below it the shapegroup's own BVH in object space.  Entering an item transforms the ray with the instance's inverse
@@ -442,34 +464,43 @@ template <bool SHADOW, bool COUNT> B2_DEV bool traverseTop(const DScene &sc, con
 // when REFILL or more lanes are idle they commit their results and pull the next rays from a global ticket counter
 // (one atomic per refill), so lanes do not idle until the slowest ray of a 32-ray batch is done.
 //   fetch(idx, o, d, mint, maxt) -> 0: nothing to do for this item, 1: ray misses the scene box (commit a miss), 2: traverse
-//   commit(idx, found, hit)
+//   commit(idx, found, hit, item): `hit` is the miss record unless something was found; `item`: the instance that was hit
+//   (traverseTop), else 0xFFFFFFFF
+// The ticket protocol lives in refillQueue alone.  A walker hands it start(lane), which sets up the walker's own state for the
+// lane's new ray, and walk(lane, exhausted), which advances the warp's lanes until enough of them finish; a finished lane sets
+// active = false and pending = true.
 // ------------------------------------------------------------------------------------------------------------
-template <bool SHADOW, bool COUNT, typename Fetch, typename Commit>
-B2_DEV void traverseQueue(const DScene &sc, const TraceMem &tm, uint32_t n, unsigned long long *ticket, Fetch fetch, Commit commit,
-                          uint32_t &nodeVisits, uint32_t &primTests) {
+struct QueueLane {
+    bool active, pending, found;
+    uint32_t best; // leaf-ordered index of the closest hit so far
+    V3 o, d, idir, ood;
+    float mint, maxt;
+    HitRec hit;
+};
+
+template <typename Fetch, typename Commit, typename Start, typename Walk>
+B2_DEV void refillQueue(const DScene &sc, uint32_t n, unsigned long long *ticket, Fetch fetch, Commit commit, Start start, Walk walk) {
     const unsigned FULL = 0xffffffffu;
     const int lane = threadIdx.x & 31;
-    const uint32_t stride = tm.stride;
-    bool active = false, pending = false, exhausted = false, found = false;
-    uint32_t idx = 0, best = 0;
-    V3 o(0.0f), d(0.0f), idir(0.0f), ood(0.0f);
-    float mint = 0, maxt = 0;
-    HitRec hit;
-    hit.t = B2_INF; hit.u = 0; hit.v = 0; hit.prim = 0xFFFFFFFFu;
-    int sp = 0, ref = 0;
+    QueueLane q;
+    q.active = false; q.pending = false; q.found = false; q.best = 0;
+    q.o = V3(0.0f); q.d = V3(0.0f); q.idir = V3(0.0f); q.ood = V3(0.0f);
+    q.mint = 0; q.maxt = 0;
+    q.hit = missHit();
+    bool exhausted = false;
+    uint32_t idx = 0;
     const int refill = (int) sc.refill;
-    const int leafVote = (int) sc.leafVote;
     // tickets a warp reserves per atomic: 128 for big launches, down to 32 so that small launches still spread over the grid
     const unsigned warpsInGrid = gridDim.x * (blockDim.x >> 5);
     const unsigned long long CHUNK = (unsigned long long) min(128u, max(32u, (n / (4u * warpsInGrid)) & ~31u));
     unsigned long long chunkNext = 0, chunkEnd = 0; // warp-uniform: locally reserved ticket range
     while (true) {
-        const unsigned idle = __ballot_sync(FULL, !active);
+        const unsigned idle = __ballot_sync(FULL, !q.active);
         if (idle == FULL || (!exhausted && __popc(idle) >= refill)) {
-            if (pending) {
-                if (found) { hit.leaf = best; hit.prim = __ldg(sc.leafPrim + best); }
-                commit(idx, found, hit);
-                pending = false;
+            if (q.pending) {
+                if (q.found) { q.hit.leaf = q.best; q.hit.prim = __ldg(sc.leafPrim + q.best); }
+                commit(idx, q.found, q.hit, 0xFFFFFFFFu);
+                q.pending = false;
             }
             if (!exhausted) {
                 const unsigned need = (unsigned) __popc(idle);
@@ -486,40 +517,49 @@ B2_DEV void traverseQueue(const DScene &sc, const TraceMem &tm, uint32_t n, unsi
                 else my = base2 + (rank - have);
                 if (have < need) { chunkNext = base2 + (need - have); chunkEnd = base2 + CHUNK; }
                 else chunkNext += need;
-                const unsigned long long base = chunkNext - need; // only used for the exhaustion test below
-                if (!active) {
-                    if (my < n) {
-                        idx = (uint32_t) my;
-                        found = false;
-                        hit.t = B2_INF; hit.u = 0; hit.v = 0; hit.prim = 0xFFFFFFFFu;
-                        const int r = fetch(idx, o, d, mint, maxt);
-                        if (r == 2) {
-                            active = true;
-                            sp = 0;
-                            ref = sc.rootRef;
-                            slabSetup(o, d, idir, ood);
-                        } else if (r == 1) pending = true;
-                    }
+                if (!q.active && my < n) {
+                    idx = (uint32_t) my;
+                    q.found = false;
+                    q.hit = missHit();
+                    const int r = fetch(idx, q.o, q.d, q.mint, q.maxt);
+                    if (r == 2) {
+                        q.active = true;
+                        slabSetup(q.o, q.d, q.idir, q.ood);
+                        start(q);
+                    } else if (r == 1) q.pending = true;
                 }
-                (void) base;
                 if (chunkNext >= n) exhausted = true; // every later ticket of this warp is out of range
             }
-            if (__ballot_sync(FULL, active) == 0) {
+            if (__ballot_sync(FULL, q.active) == 0) {
                 if (exhausted) {
-                    if (pending) { commit(idx, found, hit); pending = false; }
+                    if (q.pending) commit(idx, q.found, q.hit, 0xFFFFFFFFu);
                     break;
                 }
                 continue;
             }
         }
+        walk(q, exhausted);
+    }
+}
+
+template <bool SHADOW, bool COUNT, typename Fetch, typename Commit>
+B2_DEV void traverseQueue(const DScene &sc, const TraceMem &tm, uint32_t n, unsigned long long *ticket, Fetch fetch, Commit commit,
+                          uint32_t &nodeVisits, uint32_t &primTests) {
+    const unsigned FULL = 0xffffffffu;
+    const uint32_t stride = tm.stride;
+    int sp = 0, ref = 0;
+    const int refill = (int) sc.refill;
+    const int leafVote = (int) sc.leafVote;
+    auto start = [&](const QueueLane &) { sp = 0; ref = sc.rootRef; };
+    auto walk = [&](QueueLane &q, bool exhausted) {
         // ---- node phase ("while-while" with a vote): lanes standing on an inner node keep descending; lanes that reached
         // a leaf wait, so that the leaf code below runs with many lanes instead of 2-3.  The phase ends when enough lanes
         // wait at a leaf, nobody is on a node any more, or enough lanes went idle to make a refill worthwhile.
         while (true) {
-            const bool atNode = active && ref >= 0;
+            const bool atNode = q.active && ref >= 0;
             const unsigned nm = __ballot_sync(FULL, atNode);
             if (nm == 0) break;
-            const unsigned lm = __ballot_sync(FULL, active && ref < 0);
+            const unsigned lm = __ballot_sync(FULL, q.active && ref < 0);
             if (__popc(lm) >= leafVote) break;
             if (!exhausted && __popc(~(nm | lm)) >= refill) break;
             if (atNode) {
@@ -533,8 +573,8 @@ B2_DEV void traverseQueue(const DScene &sc, const TraceMem &tm, uint32_t n, unsi
                 }
                 if (COUNT) ++nodeVisits;
                 float tL, tR;
-                const bool hL = boxHit(a.x, a.y, a.z, a.w, b.x, b.y, ood, idir, mint, maxt, tL);
-                const bool hR = boxHit(b.z, b.w, c.x, c.y, c.z, c.w, ood, idir, mint, maxt, tR);
+                const bool hL = boxHit(a.x, a.y, a.z, a.w, b.x, b.y, q.ood, q.idir, q.mint, q.maxt, tL);
+                const bool hR = boxHit(b.z, b.w, c.x, c.y, c.z, c.w, q.ood, q.idir, q.mint, q.maxt, tR);
                 const int lref = __float_as_int(e.x), rref = __float_as_int(e.y);
                 if (hL && hR) {
                     int nearRef = lref, farRef = rref;
@@ -544,31 +584,32 @@ B2_DEV void traverseQueue(const DScene &sc, const TraceMem &tm, uint32_t n, unsi
                     ref = nearRef;
                 } else if (hL) ref = lref;
                 else if (hR) ref = rref;
-                else if (sp == 0) { active = false; pending = true; }
+                else if (sp == 0) { q.active = false; q.pending = true; }
                 else { --sp; ref = (int) tm.stack[sp * stride]; }
             }
         }
         // ---- leaf phase
-        if (active && ref < 0) {
+        if (q.active && ref < 0) {
             const uint32_t bits = ~(uint32_t) ref;
-            const uint32_t start = bits & 0x0FFFFFFFu, count = bits >> 28;
+            const uint32_t first = bits & 0x0FFFFFFFu, count = bits >> 28;
             for (uint32_t i = 0; i < count; ++i) {
-                const uint32_t ti = start + i;
+                const uint32_t ti = first + i;
                 const float4 *p = tm.gTris + 3 * (size_t) ti;
                 const float4 q0 = __ldg(p), q1 = __ldg(p + 1), q2 = __ldg(p + 2);
                 if (COUNT) ++primTests;
                 float tu, tv, tt;
-                if (B2_TRI_TEST(q0, q1, q2, o, d, mint, maxt, tu, tv, tt)) {
-                    found = true;
+                if (B2_TRI_TEST(q0, q1, q2, q.o, q.d, q.mint, q.maxt, tu, tv, tt)) {
+                    q.found = true;
                     if (SHADOW) break;
-                    hit.t = tt; hit.u = tu; hit.v = tv; best = ti;
-                    maxt = tt;
+                    q.hit.t = tt; q.hit.u = tu; q.hit.v = tv; q.best = ti;
+                    q.maxt = tt;
                 }
             }
-            if ((SHADOW && found) || sp == 0) { active = false; pending = true; }
+            if ((SHADOW && q.found) || sp == 0) { q.active = false; q.pending = true; }
             else { --sp; ref = (int) tm.stack[sp * stride]; }
         }
-    }
+    };
+    refillQueue(sc, n, ticket, fetch, commit, start, walk);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -586,71 +627,17 @@ B2_DEV float byteF(uint32_t w, int k) { return (float) ((w >> (8 * k)) & 0xFFu);
 template <bool SHADOW, bool COUNT, typename Fetch, typename Commit>
 B2_DEV void traverseQueue8(const DScene &sc, const TraceMem &tm, uint32_t n, unsigned long long *ticket, Fetch fetch, Commit commit,
                            uint32_t &nodeVisits, uint32_t &primTests) {
-    const unsigned FULL = 0xffffffffu;
-    const int lane = threadIdx.x & 31;
     const uint32_t stride = tm.stride;
-
-    bool active = false, pending = false, exhausted = false, found = false;
-    uint32_t idx = 0, best = 0;
-    V3 o(0.0f), d(0.0f), idir(0.0f), ood(0.0f);
-    float mint = 0, maxt = 0;
-    HitRec hit;
-    hit.t = B2_INF; hit.u = 0; hit.v = 0; hit.prim = 0xFFFFFFFFu; hit.leaf = 0;
     int sp = 0;
     uint32_t cur = 0, grpBase = 0, grpBits = 0, octFlip = 0;
-    const int refill = (int) sc.refill;
-    const unsigned warpsInGrid = gridDim.x * (blockDim.x >> 5);
-    const unsigned long long CHUNK = (unsigned long long) min(128u, max(32u, (n / (4u * warpsInGrid)) & ~31u));
-    unsigned long long chunkNext = 0, chunkEnd = 0; // warp-uniform: locally reserved ticket range
-    while (true) {
-        const unsigned idle = __ballot_sync(FULL, !active);
-        if (idle == FULL || (!exhausted && __popc(idle) >= refill)) {
-            if (pending) {
-                if (found) { hit.leaf = best; hit.prim = __ldg(sc.leafPrim + best); }
-                commit(idx, found, hit);
-                pending = false;
-            }
-            if (!exhausted) {
-                const unsigned need = (unsigned) __popc(idle);
-                const unsigned rank = (unsigned) __popc(idle & ((1u << lane) - 1u));
-                const unsigned long long have = chunkEnd - chunkNext;
-                unsigned long long base2 = 0;
-                if (have < need) {
-                    if (lane == 0) base2 = atomicAdd(ticket, (unsigned long long) CHUNK);
-                    base2 = __shfl_sync(FULL, base2, 0);
-                }
-                unsigned long long my;
-                if (rank < have) my = chunkNext + rank;
-                else my = base2 + (rank - have);
-                if (have < need) { chunkNext = base2 + (need - have); chunkEnd = base2 + CHUNK; }
-                else chunkNext += need;
-                if (!active) {
-                    if (my < n) {
-                        idx = (uint32_t) my;
-                        found = false;
-                        hit.t = B2_INF; hit.u = 0; hit.v = 0; hit.prim = 0xFFFFFFFFu;
-                        const int r = fetch(idx, o, d, mint, maxt);
-                        if (r == 2) {
-                            active = true;
-                            sp = 0; cur = 0; grpBits = 0;
-                            slabSetup(o, d, idir, ood);
-                            octFlip = 7u ^ ((d.x < 0 ? 1u : 0u) | (d.y < 0 ? 2u : 0u) | (d.z < 0 ? 4u : 0u));
-                        } else if (r == 1) pending = true;
-                    }
-                }
-                if (chunkNext >= n) exhausted = true; // every later ticket of this warp is out of range
-            }
-            if (__ballot_sync(FULL, active) == 0) {
-                if (exhausted) {
-                    if (pending) { commit(idx, found, hit); pending = false; }
-                    break;
-                }
-                continue;
-            }
-        }
+    auto start = [&](const QueueLane &q) {
+        sp = 0; cur = 0; grpBits = 0;
+        octFlip = 7u ^ ((q.d.x < 0 ? 1u : 0u) | (q.d.y < 0 ? 2u : 0u) | (q.d.z < 0 ? 4u : 0u));
+    };
+    auto walk = [&](QueueLane &q, bool) {
         // per-lane results of the node visit: hit internal children (visiting order), triangles of the hit leaf children
         uint32_t hmask = 0, tmask = 0, triBase = 0, imaskN = 0, childBaseN = 0;
-        if (active) {
+        if (q.active) {
             // ---- node: eight quantised child boxes ----
             float4 n0, n1, n2, n3, n4;
             if (cur < tm.stageNodes8) {
@@ -663,12 +650,12 @@ B2_DEV void traverseQueue8(const DScene &sc, const TraceMem &tm, uint32_t n, uns
             if (COUNT) ++nodeVisits;
             const uint32_t ew = __float_as_uint(n0.w);
             const uint32_t imask = ew >> 24;
-            const float ax = __uint_as_float((uint32_t) ((int) (int8_t) (ew & 0xFFu) + 127) << 23) * idir.x;
-            const float ay = __uint_as_float((uint32_t) ((int) (int8_t) ((ew >> 8) & 0xFFu) + 127) << 23) * idir.y;
-            const float az = __uint_as_float((uint32_t) ((int) (int8_t) ((ew >> 16) & 0xFFu) + 127) << 23) * idir.z;
-            const float bx = fmaf(n0.x, idir.x, -ood.x), by = fmaf(n0.y, idir.y, -ood.y), bz = fmaf(n0.z, idir.z, -ood.z);
+            const float ax = __uint_as_float((uint32_t) ((int) (int8_t) (ew & 0xFFu) + 127) << 23) * q.idir.x;
+            const float ay = __uint_as_float((uint32_t) ((int) (int8_t) ((ew >> 8) & 0xFFu) + 127) << 23) * q.idir.y;
+            const float az = __uint_as_float((uint32_t) ((int) (int8_t) ((ew >> 16) & 0xFFu) + 127) << 23) * q.idir.z;
+            const float bx = fmaf(n0.x, q.idir.x, -q.ood.x), by = fmaf(n0.y, q.idir.y, -q.ood.y), bz = fmaf(n0.z, q.idir.z, -q.ood.z);
             // byte planes: near = lo for a positive direction component, hi otherwise
-            const bool px = idir.x >= 0, py = idir.y >= 0, pz = idir.z >= 0;
+            const bool px = q.idir.x >= 0, py = q.idir.y >= 0, pz = q.idir.z >= 0;
             const uint32_t nx0 = __float_as_uint(px ? n2.x : n3.z), nx1 = __float_as_uint(px ? n2.y : n3.w);
             const uint32_t fx0 = __float_as_uint(px ? n3.z : n2.x), fx1 = __float_as_uint(px ? n3.w : n2.y);
             const uint32_t ny0 = __float_as_uint(py ? n2.z : n4.x), ny1 = __float_as_uint(py ? n2.w : n4.y);
@@ -682,8 +669,8 @@ B2_DEV void traverseQueue8(const DScene &sc, const TraceMem &tm, uint32_t n, uns
                 const float tnx = fmaf(byteF(s < 4 ? nx0 : nx1, k), ax, bx), tfx = fmaf(byteF(s < 4 ? fx0 : fx1, k), ax, bx);
                 const float tny = fmaf(byteF(s < 4 ? ny0 : ny1, k), ay, by), tfy = fmaf(byteF(s < 4 ? fy0 : fy1, k), ay, by);
                 const float tnz = fmaf(byteF(s < 4 ? nz0 : nz1, k), az, bz), tfz = fmaf(byteF(s < 4 ? fz0 : fz1, k), az, bz);
-                const float tmin = fmaxf(fmaxf(tnx, tny), fmaxf(tnz, mint));
-                const float tmax = fminf(fminf(tfx, tfy), fminf(tfz, maxt));
+                const float tmin = fmaxf(fmaxf(tnx, tny), fmaxf(tnz, q.mint));
+                const float tmax = fminf(fminf(tfx, tfy), fminf(tfz, q.maxt));
                 const uint32_t m = ((s < 4 ? meta0 : meta1) >> (8 * k)) & 0xFFu;
                 if (tmin <= tmax * 1.0000003f) {
                     if ((imask >> s) & 1u) hmask |= 1u << (24u + ((uint32_t) s ^ octFlip));
@@ -705,25 +692,25 @@ B2_DEV void traverseQueue8(const DScene &sc, const TraceMem &tm, uint32_t n, uns
                 const float4 q0 = __ldg(p), q1 = __ldg(p + 1), q2 = __ldg(p + 2);
                 if (COUNT) ++primTests;
                 float tu, tv, tt;
-                if (B2_TRI_TEST(q0, q1, q2, o, d, mint, maxt, tu, tv, tt)) {
-                    found = true;
+                if (B2_TRI_TEST(q0, q1, q2, q.o, q.d, q.mint, q.maxt, tu, tv, tt)) {
+                    q.found = true;
                     if (SHADOW) break;
-                    hit.t = tt; hit.u = tu; hit.v = tv; best = ti;
-                    maxt = tt;
+                    q.hit.t = tt; q.hit.u = tu; q.hit.v = tv; q.best = ti;
+                    q.maxt = tt;
                 }
             }
             // ---- next node ----
-            if (SHADOW && found) { active = false; pending = true; }
+            if (SHADOW && q.found) { q.active = false; q.pending = true; }
             else {
                 if (hmask) {
                     if (grpBits >> 24) { tm.stack8[sp * stride] = make_uint2(grpBase, grpBits); ++sp; }
                     grpBase = childBaseN; grpBits = hmask | imaskN;
                 }
                 if (!(grpBits >> 24)) {
-                    if (sp == 0) { active = false; pending = true; }
+                    if (sp == 0) { q.active = false; q.pending = true; }
                     else { --sp; const uint2 g = tm.stack8[sp * stride]; grpBase = g.x; grpBits = g.y; }
                 }
-                if (active) {
+                if (q.active) {
                     const uint32_t b = 31u - (uint32_t) __clz((int) grpBits);
                     grpBits &= ~(1u << b);
                     const uint32_t slot = (b - 24u) ^ octFlip;
@@ -731,7 +718,39 @@ B2_DEV void traverseQueue8(const DScene &sc, const TraceMem &tm, uint32_t n, uns
                 }
             }
         }
-    }
+    };
+    refillQueue(sc, n, ticket, fetch, commit, start, walk);
+}
+
+// The tree the ray-query kernels (k_extend, k_occluded, k_trace_rays) walk, which also fixes their shared-memory layout: the 8-wide tree
+// of a non-instanced BVH scene when the commit kept it (it drops it when it is too deep for the wide stack), else the binary layout (the
+// binary tree, the two levels of an instanced scene, the flat leaf).  The flat-leaf kernels and volpath name their walker themselves.
+enum Walker { WALK_FLAT, WALK_BINARY, WALK_WIDE };
+B2_DEV Walker traceWalker(const DScene &sc) { return sc.nodes8 != nullptr && !sc.rootCount && !sc.nItems ? WALK_WIDE : WALK_BINARY; }
+
+// The ray queries of a launch: items [0, n), each traced with the fetch / commit contract above.  BVH scenes take the queue of their
+// tree; instanced scenes and the flat leaf take a static grid-stride loop (per-lane tickets were slower for instanced scenes,
+// DESIGN.md §8c).
+template <bool SHADOW, bool COUNT, typename Fetch, typename Commit>
+B2_DEV void traceQueue(const DScene &sc, const TraceMem &tm, uint32_t n, unsigned long long *ticket, Fetch fetch, Commit commit,
+                       uint32_t &nodeVisits, uint32_t &primTests) {
+    if (traceWalker(sc) == WALK_WIDE) traverseQueue8<SHADOW, COUNT>(sc, tm, n, ticket, fetch, commit, nodeVisits, primTests);
+    else if (!sc.rootCount && !sc.nItems) traverseQueue<SHADOW, COUNT>(sc, tm, n, ticket, fetch, commit, nodeVisits, primTests);
+    else
+        for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {
+            const uint32_t i = base + threadIdx.x;
+            V3 o, d;
+            float mint, maxt;
+            const int r = i < n ? fetch(i, o, d, mint, maxt) : 0;
+            if (r == 0) continue;
+            HitRec h = missHit();
+            uint32_t item = 0xFFFFFFFFu;
+            bool found = false;
+            if (r == 2)
+                found = sc.nItems ? traverseTop<SHADOW, COUNT>(sc, tm, o, d, mint, maxt, h, item, nodeVisits, primTests)
+                                  : traverseFlat<SHADOW, COUNT>(sc, tm, o, d, mint, maxt, h, primTests);
+            commit(i, found, h, item);
+        }
 }
 
 } // namespace b2

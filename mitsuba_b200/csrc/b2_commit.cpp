@@ -261,22 +261,17 @@ struct Accel {
     double ms = 0;                    // b2_stats::accel_build_ms: the world and shapegroup builds
     size_t uploadBytes = 0;           // the builds' share of b2_stats::bytes_uploaded
 };
-// A host-built tree moved to the device: its node arrays are copied on `st` (pageable sources are staged before the copy returns, so `h`
-// may go at once; the caller synchronises `st` before the arrays are read elsewhere), its leaf order is taken over.
-template <typename T> static cudaError_t toDevice(const std::vector<T> &v, T *&d, cudaStream_t st) {
-    if (v.empty()) return cudaSuccess;
-    T *p = nullptr;
-    const cudaError_t e = cudaMalloc((void **) &p, v.size() * sizeof(T));
-    if (e != cudaSuccess) return e;
-    d = p;
-    return cudaMemcpyAsync(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, st);
-}
+// A host-built tree moved to the device: its node arrays are uploaded on `st` (`h` may go at once; the caller synchronises `st` before
+// the arrays are read elsewhere), its leaf order is taken over.
 static cudaError_t uploadTree(BVHResult &h, cudaStream_t st, DeviceBVHResult &out) {
     out.leafPrims.swap(h.leafPrims);
     out.rootRef = h.rootRef; out.depth = h.depth; out.depth8 = h.depth8;
     out.nNodes = h.nodes.size(); out.nNodes8 = h.nodes8.size();
-    cudaError_t e = toDevice(h.nodes, out.nodes, st);
-    if (e == cudaSuccess) e = toDevice(h.nodes8, out.nodes8, st);
+    DevBuf<BVHNode> nodes;
+    DevBuf<BVH8Node> nodes8;
+    cudaError_t e = nodes.upload(h.nodes, st);
+    if (e == cudaSuccess) e = nodes8.upload(h.nodes8, st);
+    out.nodes = nodes.detach(); out.nodes8 = nodes8.detach();
     return e;
 }
 // The world or a shapegroup tree, from the builder the scene chose; the only place that looks at it.  Host: buildBVH, then uploaded
@@ -567,7 +562,7 @@ static int uploadMaterials(b2_scene *s) {
                 return fail(s->ctx, B2_ERR_INVALID, "Shape has an index-matched BSDF and an emitter attachment. This is not allowed!"); // shape.cpp:76-78
         } else s->classPresent[t] = true;
     }
-    CK(s->ctx, s->dMaterials.upload(dm));
+    CK(s->ctx, s->dMaterials.upload(dm, s->ctx->stream));
     return B2_OK;
 }
 // ---- bitmap textures and the environment map: MIP pyramids (host, as the reference builds them at load time) on the device ----
@@ -605,10 +600,10 @@ static int uploadTextures(b2_scene *s) {
         d.bsdfScale = ht.mip.maximum > 1.0f ? 0.99f * (1.0f / ht.mip.maximum) : 1.0f; // bsdf.cpp:93-107
         s->dTexData.emplace_back(new DevBuf<float>());
         const std::vector<float> packed = packPyramid(ht.mip, t.channels, d);
-        CK(ctx, s->dTexData.back()->upload(packed));
+        CK(ctx, s->dTexData.back()->upload(packed, ctx->stream));
         d.data = s->dTexData.back()->p;
     }
-    CK(ctx, s->dTextures.upload(dtex));
+    CK(ctx, s->dTextures.upload(dtex, ctx->stream));
     return B2_OK;
 }
 // Environment map: pyramid (half-rounded floats, RGB padded to float4) + the tables of EnvironmentMap::configure (envmap.cpp:260-329).
@@ -656,11 +651,11 @@ static int uploadEnvmap(b2_scene *s) {
     de.pixelSizeX = 2 * kPi / w; de.pixelSizeY = kPi / h;
     de.scale = he.scale; de.w = w; de.h = h;
     for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) { de.toWorld[3 * r + c] = he.toWorld[4 * r + c]; de.toLocal[3 * r + c] = he.toLocal[4 * r + c]; }
-    CK(ctx, s->dEnvTexels.upload(packed));
-    CK(ctx, s->dEnvCdfRows.upload(cdfRows)); CK(ctx, s->dEnvCdfCols.upload(cdfCols)); CK(ctx, s->dEnvRowWeights.upload(rowWeights));
+    CK(ctx, s->dEnvTexels.upload(packed, ctx->stream));
+    CK(ctx, s->dEnvCdfRows.upload(cdfRows, ctx->stream)); CK(ctx, s->dEnvCdfCols.upload(cdfCols, ctx->stream)); CK(ctx, s->dEnvRowWeights.upload(rowWeights, ctx->stream));
     d.data = s->dEnvTexels.p;
     de.cdfRows = s->dEnvCdfRows.p; de.cdfCols = s->dEnvCdfCols.p; de.rowWeights = s->dEnvRowWeights.p;
-    CK(ctx, s->dEnvMap.upload(std::vector<DEnvMap>(1, de)));
+    CK(ctx, s->dEnvMap.upload(std::vector<DEnvMap>(1, de), ctx->stream));
     return B2_OK;
 }
 // ---- media (volpath): the media table and the per-prim (interior, exterior) ids, none when no mesh borders a medium ----
@@ -678,7 +673,7 @@ static int uploadMedia(b2_scene *s, size_t nPrims) {
         memcpy(d.albedo, m.albedo, 12); memcpy(d.res, m.res, 12); memcpy(d.worldToGrid, m.world_to_grid, 48);
         memcpy(d.aabbMin, m.aabb_min, 12); memcpy(d.aabbMax, m.aabb_max, 12);
         s->dDensity.emplace_back(new DevBuf<float>());
-        CK(s->ctx, s->dDensity.back()->upload(s->media[i].density));
+        CK(s->ctx, s->dDensity.back()->upload(s->media[i].density, s->ctx->stream));
         d.density = s->dDensity.back()->p;
     }
     std::vector<int2> primMedia;
@@ -689,8 +684,8 @@ static int uploadMedia(b2_scene *s, size_t nPrims) {
         for (auto &m : s->meshes)
             for (size_t j = 0; j < m.idx.size() / 3; ++j) primMedia[m.primOffset + j] = make_int2(m.interior, m.exterior);
     }
-    CK(s->ctx, s->dMedia.upload(dmed));
-    CK(s->ctx, s->dPrimMedia.upload(primMedia));
+    CK(s->ctx, s->dMedia.upload(dmed, s->ctx->stream));
+    CK(s->ctx, s->dPrimMedia.upload(primMedia, s->ctx->stream));
     return B2_OK;
 }
 // ---- emitters in device order, their CDF and the triangle CDF of each area emitter: scene.cpp:375-380, trimesh.cpp:388-403, pmf.h.
@@ -738,9 +733,9 @@ static int uploadEmitters(b2_scene *s, const std::vector<int> &emOrder, float &e
             emCdf.back() = 1.0f;
         }
     }
-    CK(s->ctx, s->dEmitters.upload(de));
-    CK(s->ctx, s->dEmitterCdf.upload(emCdf));
-    CK(s->ctx, s->dTriCdf.upload(triCdf));
+    CK(s->ctx, s->dEmitters.upload(de, s->ctx->stream));
+    CK(s->ctx, s->dEmitterCdf.upload(emCdf, s->ctx->stream));
+    CK(s->ctx, s->dTriCdf.upload(triCdf, s->ctx->stream));
     return B2_OK;
 }
 // ---- camera ----
@@ -767,15 +762,15 @@ static void fillCamera(const b2_scene *s, DCamera &cam) {
 // ---- the device scene: the remaining uploads, DScene over the scene's device arrays, launch configurations, b2_stats ----
 static int assembleScene(b2_scene *s, const Flat &f, const Accel &a, const LeafRows &rows, const FlatLeaf &fl, const std::vector<int> &emIndex, float emNorm) {
     b2_ctx *ctx = s->ctx;
-    CK(ctx, s->dTriAccel.upload(rows.tri));
-    CK(ctx, s->dTriPlane.upload(rows.plane));
-    CK(ctx, s->dLeafPrim.upload(a.leafPrims));
-    CK(ctx, s->dFlatRec.upload(fl.rec));
-    CK(ctx, s->dFlatIdx.upload(fl.idx));
-    CK(ctx, s->dVerts.upload(f.verts));
-    CK(ctx, s->dNorms.upload(f.norms));
-    CK(ctx, s->dTexc.upload(f.texc));
-    CK(ctx, s->dInstances.upload(a.items));
+    CK(ctx, s->dTriAccel.upload(rows.tri, ctx->stream));
+    CK(ctx, s->dTriPlane.upload(rows.plane, ctx->stream));
+    CK(ctx, s->dLeafPrim.upload(a.leafPrims, ctx->stream));
+    CK(ctx, s->dFlatRec.upload(fl.rec, ctx->stream));
+    CK(ctx, s->dFlatIdx.upload(fl.idx, ctx->stream));
+    CK(ctx, s->dVerts.upload(f.verts, ctx->stream));
+    CK(ctx, s->dNorms.upload(f.norms, ctx->stream));
+    CK(ctx, s->dTexc.upload(f.texc, ctx->stream));
+    CK(ctx, s->dInstances.upload(a.items, ctx->stream));
     const size_t nPrims = f.nPrims, nNodes = s->dNodes.n, nNodes8 = s->dNodes8.n;
     DScene &ds = s->ds;
     memset(&ds, 0, sizeof(ds));
@@ -872,7 +867,7 @@ extern "C" int b2_scene_commit(b2_scene *s) {
     if (!s->textures.empty() || s->envmap) {
         std::vector<float> lut(64);
         b2host::ewaWeightTable(lut.data());
-        CK(ctx, s->dEwaLut.upload(lut));
+        CK(ctx, s->dEwaLut.upload(lut, ctx->stream));
     }
     if (int rc = uploadMedia(s, flat.nPrims)) return rc;
     clk.mark("materials / textures / media");
@@ -880,6 +875,7 @@ extern "C" int b2_scene_commit(b2_scene *s) {
     if (int rc = uploadEmitters(s, emo.order, emNorm)) return rc;
     clk.mark("emitters");
     if (int rc = assembleScene(s, flat, acc, rows, fl, emo.index, emNorm)) return rc;
+    CK(ctx, cudaStreamSynchronize(ctx->stream)); // the uploads of the stages above
     clk.mark("upload");
     s->committed = true;
     return B2_OK;

@@ -97,6 +97,7 @@ extern "C" int b2_context_create(int device, b2_ctx **out) {
     }
     vdc.resize(26 * 52, 0);
     ctx->hVdc = vdc; ctx->hInv = inv;
+    const cudaStream_t st = ctx->stream;
     {   // nibble-sliced direction matrices: nib[d][p][v] = XOR_{k in bits(v)} m32[d][4p + k]  (b2_sampler.cuh: sobolSampleNib)
         std::vector<uint32_t> nib((size_t) 1024 * 13 * 16, 0u);
         for (int d = 0; d < 1024; ++d)
@@ -108,16 +109,17 @@ extern "C" int b2_context_create(int device, b2_ctx **out) {
                     nib[((size_t) d * 13 + p) * 16 + v] = x;
                 }
         if (cudaMalloc((void **) &ctx->dNib, nib.size() * 4) != cudaSuccess ||
-            cudaMemcpy(ctx->dNib, nib.data(), nib.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) {
+            cudaMemcpyAsync(ctx->dNib, nib.data(), nib.size() * 4, cudaMemcpyHostToDevice, st) != cudaSuccess) {
             b2_context_destroy(ctx);
             return fail(nullptr, B2_ERR_CUDA, "b2_context_create: upload of the Sobol' nibble tables failed");
         }
     }
     if (cudaMalloc((void **) &ctx->dM32, m32.size() * 4) != cudaSuccess || cudaMalloc((void **) &ctx->dVdc, vdc.size() * 8) != cudaSuccess ||
         cudaMalloc((void **) &ctx->dInv, inv.size() * 8) != cudaSuccess ||
-        cudaMemcpy(ctx->dM32, m32.data(), m32.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
-        cudaMemcpy(ctx->dVdc, vdc.data(), vdc.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess ||
-        cudaMemcpy(ctx->dInv, inv.data(), inv.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) {
+        cudaMemcpyAsync(ctx->dM32, m32.data(), m32.size() * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(ctx->dVdc, vdc.data(), vdc.size() * 8, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(ctx->dInv, inv.data(), inv.size() * 8, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess) {
         b2_context_destroy(ctx);
         return fail(nullptr, B2_ERR_CUDA, "b2_context_create: upload of the Sobol' tables failed");
     }
@@ -589,7 +591,8 @@ static int fillRender(b2_scene *s, const b2_render_params *p, DRender &r) {
                 lut[(size_t) (13 + q) * 16 + v] = b;
             }
         if (s->dLookupNib.alloc(lut.size()) != cudaSuccess) return fail(ctx, B2_ERR_CUDA, "cudaMalloc(lookup tables) failed");
-        if (cudaMemcpy(s->dLookupNib.p, lut.data(), lut.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) return fail(ctx, B2_ERR_CUDA, "upload of lookup tables failed");
+        if (cudaMemcpyAsync(s->dLookupNib.p, lut.data(), lut.size() * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)
+            return fail(ctx, B2_ERR_CUDA, "upload of lookup tables failed");
         r.lookupNib = s->dLookupNib.p;
     }
     return B2_OK;
@@ -916,22 +919,36 @@ extern "C" int b2_film_develop(const float *film, int W, int H, float *rgb) { //
 // ------------------------------------------------------------------------------------------------
 // component entry points
 // ------------------------------------------------------------------------------------------------
-struct TmpDev {
-    std::vector<void *> ptrs;
-    ~TmpDev() { for (void *p : ptrs) cudaFree(p); }
-    template <typename T> T *alloc(size_t n) {
-        void *p = nullptr;
-        if (cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return nullptr;
-        ptrs.push_back(p);
-        return (T *) p;
-    }
-    template <typename T> T *upload(const T *h, size_t n) {
-        T *d = alloc<T>(n);
-        if (d && n) cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice);
-        return d;
-    }
-};
 #define NEED_COMMIT(s) if (!(s) || !(s)->committed) return fail((s) ? (s)->ctx : nullptr, B2_ERR_INVALID, "scene not committed")
+
+// A host array of floats that a component call reads (In) or writes (Out).
+struct In { const float *p; size_t n; };
+struct Out { float *p; size_t n; };
+// The call path of the component entry points: refuses a null array that is not empty, allocates a device buffer per array, queues the
+// uploads, runs launch(d) with the device arrays (the inputs, then the outputs, each in the order given), checks the launch, queues the
+// read-backs and synchronises once.  The buffers are freed on every return.
+template <typename Launch>
+static int componentCall(b2_ctx *ctx, const char *name, const std::vector<In> &in, const std::vector<Out> &out, Launch &&launch) {
+    for (const In &a : in) if (!a.p && a.n) return fail(ctx, B2_ERR_INVALID, std::string(name) + ": null argument");
+    for (const Out &a : out) if (!a.p && a.n) return fail(ctx, B2_ERR_INVALID, std::string(name) + ": null argument");
+    CK(ctx, cudaSetDevice(ctx->device));
+    const cudaStream_t st = ctx->stream;
+    std::vector<DevBuf<float>> buf(in.size() + out.size());
+    std::vector<float *> d(buf.size());
+    for (size_t k = 0; k < buf.size(); ++k) {
+        if (buf[k].alloc(std::max<size_t>(k < in.size() ? in[k].n : out[k - in.size()].n, 1)) != cudaSuccess)
+            return fail(ctx, B2_ERR_CUDA, std::string(name) + ": device allocation failed");
+        d[k] = buf[k].p;
+    }
+    for (size_t k = 0; k < in.size(); ++k)
+        if (in[k].n) CK(ctx, cudaMemcpyAsync(d[k], in[k].p, in[k].n * sizeof(float), cudaMemcpyHostToDevice, st));
+    launch(d.data());
+    CK(ctx, cudaGetLastError());
+    for (size_t k = 0; k < out.size(); ++k)
+        if (out[k].n) CK(ctx, cudaMemcpyAsync(out[k].p, d[in.size() + k], out[k].n * sizeof(float), cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    return B2_OK;
+}
 
 extern "C" int b2_trace_device(b2_scene *s, uint64_t n, const float *d_rays, int mode, int parity_mode, float *d_tuvp, float *ms_kernel) {
     NEED_COMMIT(s);
@@ -944,21 +961,22 @@ extern "C" int b2_trace_device(b2_scene *s, uint64_t n, const float *d_rays, int
     struct EventPair { cudaEvent_t a = nullptr, b = nullptr; ~EventPair() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); } } ev;
     CK(ctx, cudaEventCreate(&ev.a));
     CK(ctx, cudaEventCreate(&ev.b));
-    cudaEvent_t a = ev.a, b = ev.b;
-    if (count) cudaMemsetAsync(s->dCounters.p + CTR_NODEVIS, 0, 16, st);
-    cudaMemsetAsync(s->dCounters.p + CTR_TICKET_EXT, 0, 8, st);
+    if (count) CK(ctx, cudaMemsetAsync(s->dCounters.p + CTR_NODEVIS, 0, 16, st));
+    CK(ctx, cudaMemsetAsync(s->dCounters.p + CTR_TICKET_EXT, 0, 8, st));
     const Kernels kn = kernelsFor(s, parity_mode != 0);
-    cudaEventRecord(a, st);
-    kn.set.trace(kn.cfg, s->ds, (const float4 *) d_rays, (float4 *) d_tuvp, n, shadow, count, s->dCounters.p, st);
-    cudaEventRecord(b, st);
-    CK(ctx, cudaStreamSynchronize(st));
-    CK(ctx, cudaGetLastError());
+    // the events bracket the kernel alone: ms_kernel is the `traversal` figure of bench.py
+    if (int rc = componentCall(ctx, "b2_trace_device", {}, {}, [&](float *const *) {
+            cudaEventRecord(ev.a, st);
+            kn.set.trace(kn.cfg, s->ds, (const float4 *) d_rays, (float4 *) d_tuvp, n, shadow, count, s->dCounters.p, st);
+            cudaEventRecord(ev.b, st);
+        }))
+        return rc;
     float ms = 0;
-    cudaEventElapsedTime(&ms, a, b);
+    cudaEventElapsedTime(&ms, ev.a, ev.b);
     if (ms_kernel) *ms_kernel = ms;
     if (count) {
         unsigned long long c[2];
-        cudaMemcpy(c, s->dCounters.p + CTR_NODEVIS, 16, cudaMemcpyDeviceToHost);
+        CK(ctx, cudaMemcpy(c, s->dCounters.p + CTR_NODEVIS, 16, cudaMemcpyDeviceToHost));
         s->stats.node_visits = c[0]; s->stats.prim_tests = c[1];
     }
     return B2_OK;
@@ -966,16 +984,13 @@ extern "C" int b2_trace_device(b2_scene *s, uint64_t n, const float *d_rays, int
 extern "C" int b2_trace(b2_scene *s, uint64_t n, const float *rays, int mode, int parity_mode, float *t, float *u, float *v, uint32_t *prim,
                         float *ms_kernel) {
     NEED_COMMIT(s);
-    b2_ctx *ctx = s->ctx;
-    CK(ctx, cudaSetDevice(ctx->device));
-    TmpDev tmp;
-    float *dR = tmp.upload(rays, 8 * n);
-    float *dO = tmp.alloc<float>(4 * n);
-    if (!dR || !dO) return fail(ctx, B2_ERR_CUDA, "b2_trace: device allocation failed");
-    int rc = b2_trace_device(s, n, dR, mode, parity_mode, dO, ms_kernel);
-    if (rc) return rc;
+    if (n > 0xFFFFFFFFull) return fail(s->ctx, B2_ERR_INVALID, "b2_trace: at most 2^32-1 rays per call");
     std::vector<float> h(4 * n);
-    CK(ctx, cudaMemcpy(h.data(), dO, 4 * n * sizeof(float), cudaMemcpyDeviceToHost));
+    int rc = B2_OK;
+    if (int e = componentCall(s->ctx, "b2_trace", {{rays, 8 * n}}, {{h.data(), 4 * n}},
+                              [&](float *const *d) { rc = b2_trace_device(s, n, d[0], mode, parity_mode, d[1], ms_kernel); }))
+        return e;
+    if (rc) return rc;
     for (uint64_t i = 0; i < n; ++i) {
         if (t) t[i] = h[4 * i];
         if (u) u[i] = h[4 * i + 1];
@@ -986,135 +1001,85 @@ extern "C" int b2_trace(b2_scene *s, uint64_t n, const float *rays, int mode, in
 }
 extern "C" int b2_bsdf_eval(b2_scene *s, int mat, uint64_t n, const float *wi, const float *wo, int parity_mode, float *out_rgb, float *out_pdf) {
     NEED_COMMIT(s);
-    b2_ctx *ctx = s->ctx;
-    if (mat < 0 || mat >= (int) s->materials.size()) return fail(ctx, B2_ERR_INVALID, "invalid material id");
-    CK(ctx, cudaSetDevice(ctx->device));
-    TmpDev tmp;
-    float *dWi = tmp.upload(wi, 3 * n), *dWo = tmp.upload(wo, 3 * n), *dRgb = tmp.alloc<float>(3 * n), *dPdf = tmp.alloc<float>(n);
+    if (mat < 0 || mat >= (int) s->materials.size()) return fail(s->ctx, B2_ERR_INVALID, "invalid material id");
     const Kernels kn = kernelsFor(s, parity_mode != 0);
-    kn.set.bsdf_eval(kn.cfg, s->ds, mat, n, dWi, dWo, dRgb, dPdf, ctx->stream);
-    CK(ctx, cudaStreamSynchronize(ctx->stream));
-    CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(out_rgb, dRgb, 3 * n * sizeof(float), cudaMemcpyDeviceToHost));
-    CK(ctx, cudaMemcpy(out_pdf, dPdf, n * sizeof(float), cudaMemcpyDeviceToHost));
-    return B2_OK;
+    return componentCall(s->ctx, "b2_bsdf_eval", {{wi, 3 * n}, {wo, 3 * n}}, {{out_rgb, 3 * n}, {out_pdf, n}},
+                         [&](float *const *d) { kn.set.bsdf_eval(kn.cfg, s->ds, mat, n, d[0], d[1], d[2], d[3], s->ctx->stream); });
 }
 extern "C" int b2_bsdf_sample(b2_scene *s, int mat, uint64_t n, const float *wi, const float *samples, int parity_mode, float *out) {
     NEED_COMMIT(s);
-    b2_ctx *ctx = s->ctx;
-    if (mat < 0 || mat >= (int) s->materials.size()) return fail(ctx, B2_ERR_INVALID, "invalid material id");
-    CK(ctx, cudaSetDevice(ctx->device));
-    TmpDev tmp;
-    float *dWi = tmp.upload(wi, 3 * n), *dS = tmp.upload(samples, 3 * n), *dO = tmp.alloc<float>(10 * n);
+    if (mat < 0 || mat >= (int) s->materials.size()) return fail(s->ctx, B2_ERR_INVALID, "invalid material id");
     const Kernels kn = kernelsFor(s, parity_mode != 0);
-    kn.set.bsdf_sample(kn.cfg, s->ds, mat, n, dWi, dS, dO, ctx->stream);
-    CK(ctx, cudaStreamSynchronize(ctx->stream));
-    CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(out, dO, 10 * n * sizeof(float), cudaMemcpyDeviceToHost));
-    return B2_OK;
+    return componentCall(s->ctx, "b2_bsdf_sample", {{wi, 3 * n}, {samples, 3 * n}}, {{out, 10 * n}},
+                         [&](float *const *d) { kn.set.bsdf_sample(kn.cfg, s->ds, mat, n, d[0], d[1], d[2], s->ctx->stream); });
 }
 extern "C" int b2_sample_emitter_direct(b2_scene *s, uint64_t n, const float *ref, const float *samples, int parity_mode, float *out) {
     NEED_COMMIT(s);
-    b2_ctx *ctx = s->ctx;
-    if (s->emitters.empty()) return fail(ctx, B2_ERR_INVALID, "scene has no emitters");
-    CK(ctx, cudaSetDevice(ctx->device));
-    TmpDev tmp;
-    float *dR = tmp.upload(ref, 6 * n), *dS = tmp.upload(samples, 2 * n), *dO = tmp.alloc<float>(12 * n);
+    if (s->emitters.empty()) return fail(s->ctx, B2_ERR_INVALID, "scene has no emitters");
     const Kernels kn = kernelsFor(s, parity_mode != 0);
-    kn.set.emitter_direct(kn.cfg, s->ds, n, dR, dS, dO, ctx->stream);
-    CK(ctx, cudaStreamSynchronize(ctx->stream));
-    CK(ctx, cudaGetLastError());
-    std::vector<float> h(12 * n);
-    CK(ctx, cudaMemcpy(h.data(), dO, 12 * n * sizeof(float), cudaMemcpyDeviceToHost));
+    if (int rc = componentCall(s->ctx, "b2_sample_emitter_direct", {{ref, 6 * n}, {samples, 2 * n}}, {{out, 12 * n}},
+                               [&](float *const *d) { kn.set.emitter_direct(kn.cfg, s->ds, n, d[0], d[1], d[2], s->ctx->stream); }))
+        return rc;
     // fold the visibility test (scene.cpp:838-843) into `visible` with the occlusion kernel
     std::vector<float> rays(8 * n);
     for (uint64_t i = 0; i < n; ++i) {
         float *r = &rays[8 * i];
         r[0] = ref[6 * i]; r[1] = ref[6 * i + 1]; r[2] = ref[6 * i + 2]; r[3] = 1e-4f;
-        r[4] = h[12 * i]; r[5] = h[12 * i + 1]; r[6] = h[12 * i + 2]; r[7] = h[12 * i + 3] * (1 - 1e-3f);
+        r[4] = out[12 * i]; r[5] = out[12 * i + 1]; r[6] = out[12 * i + 2]; r[7] = out[12 * i + 3] * (1 - 1e-3f);
     }
     std::vector<uint32_t> occ(n);
-    int rc = b2_trace(s, n, rays.data(), 1, parity_mode, nullptr, nullptr, nullptr, occ.data(), nullptr);
-    if (rc) return rc;
+    if (int rc = b2_trace(s, n, rays.data(), 1, parity_mode, nullptr, nullptr, nullptr, occ.data(), nullptr)) return rc;
     for (uint64_t i = 0; i < n; ++i) {
-        if (h[12 * i + 8] != 0 && occ[i]) { h[12 * i + 8] = 0; h[12 * i + 4] = 0; h[12 * i + 5] = h[12 * i + 6] = h[12 * i + 7] = 0; }
-        else if (h[12 * i + 8] == 0) { h[12 * i + 4] = 0; }
+        float *o = &out[12 * i];
+        if (o[8] != 0 && occ[i]) { o[8] = 0; o[4] = 0; o[5] = o[6] = o[7] = 0; }
+        else if (o[8] == 0) { o[4] = 0; }
     }
-    memcpy(out, h.data(), 12 * n * sizeof(float));
     return B2_OK;
 }
 // Medium component probe (parity tests): what = 0 evalTransmittance (in: n x 8 ray floats, out n x 3), 1 sampleDistance (out n x 12),
 // 2 density lookup (in n x 3, out n), 3 phase sample (in n x 5: wi, two uniforms; out n x 5: wo, pdf, eval)
 extern "C" int b2_medium_probe(b2_scene *s, int medium, int what, uint64_t n, const float *in, uint64_t seed, int parity_mode, float *out) {
     NEED_COMMIT(s);
-    b2_ctx *ctx = s->ctx;
-    if (medium < 0 || medium >= (int) s->media.size()) return fail(ctx, B2_ERR_INVALID, "invalid medium id");
-    if (what < 0 || what > 3 || !in || !out) return fail(ctx, B2_ERR_INVALID, "b2_medium_probe: invalid argument");
+    if (medium < 0 || medium >= (int) s->media.size()) return fail(s->ctx, B2_ERR_INVALID, "invalid medium id");
+    if (what < 0 || what > 3 || !in || !out) return fail(s->ctx, B2_ERR_INVALID, "b2_medium_probe: invalid argument");
     static const int inW[4] = {8, 8, 3, 5}, outW[4] = {3, 12, 1, 5};
-    CK(ctx, cudaSetDevice(ctx->device));
-    TmpDev tmp;
-    float *dI = tmp.upload(in, (size_t) inW[what] * n), *dO = tmp.alloc<float>((size_t) outW[what] * n);
     const Kernels kn = kernelsFor(s, parity_mode != 0);
-    kn.set.medium_probe(kn.cfg, s->ds, medium, what, n, dI, seed, dO, ctx->stream);
-    CK(ctx, cudaStreamSynchronize(ctx->stream));
-    CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(out, dO, (size_t) outW[what] * n * sizeof(float), cudaMemcpyDeviceToHost));
-    return B2_OK;
+    return componentCall(s->ctx, "b2_medium_probe", {{in, inW[what] * n}}, {{out, outW[what] * n}},
+                         [&](float *const *d) { kn.set.medium_probe(kn.cfg, s->ds, medium, what, n, d[0], seed, d[1], s->ctx->stream); });
 }
 // Texture probes (parity tests)
 extern "C" int b2_texture_eval(b2_scene *s, int texture_id, uint64_t n, const float *uv, const float *partials, int parity_mode, float *out) {
     NEED_COMMIT(s);
-    b2_ctx *ctx = s->ctx;
-    if (texture_id < 0 || texture_id >= (int) s->textures.size()) return fail(ctx, B2_ERR_INVALID, "invalid texture id");
-    if (!uv || !out) return fail(ctx, B2_ERR_INVALID, "b2_texture_eval: null argument");
+    if (texture_id < 0 || texture_id >= (int) s->textures.size()) return fail(s->ctx, B2_ERR_INVALID, "invalid texture id");
+    if (!uv || !out) return fail(s->ctx, B2_ERR_INVALID, "b2_texture_eval: null argument");
     std::vector<float> in(6 * n, 0.0f);
     for (uint64_t i = 0; i < n; ++i) {
         in[6 * i] = uv[2 * i]; in[6 * i + 1] = uv[2 * i + 1];
         if (partials) for (int k = 0; k < 4; ++k) in[6 * i + 2 + k] = partials[4 * i + k];
     }
-    CK(ctx, cudaSetDevice(ctx->device));
-    TmpDev tmp;
-    float *dI = tmp.upload(in.data(), 6 * n), *dO = tmp.alloc<float>(3 * n);
     const Kernels kn = kernelsFor(s, parity_mode != 0);
-    kn.set.texture_probe(kn.cfg, s->ds, 0, texture_id, partials ? 1 : 0, 1.0f, n, dI, dO, ctx->stream);
-    CK(ctx, cudaStreamSynchronize(ctx->stream));
-    CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(out, dO, 3 * n * sizeof(float), cudaMemcpyDeviceToHost));
-    return B2_OK;
+    return componentCall(s->ctx, "b2_texture_eval", {{in.data(), 6 * n}}, {{out, 3 * n}}, [&](float *const *d) {
+        kn.set.texture_probe(kn.cfg, s->ds, 0, texture_id, partials ? 1 : 0, 1.0f, n, d[0], d[1], s->ctx->stream);
+    });
 }
 // Probes of the committed environment map (tests): what 0 = Scene::evalEnvironment for n directions (in 3n -> out 3n), 1 = the same for sensor
 // rays with differential directions (in 9n: d, rxD, ryD -> out 3n), 2 = Scene::pdfEmitterDirect of the map for n directions (in 3n -> out n)
 extern "C" int b2_envmap_probe(b2_scene *s, int what, uint64_t n, const float *in, int parity_mode, float *out) {
     NEED_COMMIT(s);
-    b2_ctx *ctx = s->ctx;
-    if (!s->envmap) return fail(ctx, B2_ERR_INVALID, "b2_envmap_probe: the scene has no environment map");
-    if (!in || !out || what < 0 || what > 2) return fail(ctx, B2_ERR_INVALID, "b2_envmap_probe: invalid argument");
-    CK(ctx, cudaSetDevice(ctx->device));
-    TmpDev tmp;
-    const size_t nin = (what == 1 ? 9 : 3) * n, nout = (what == 2 ? 1 : 3) * n;
-    float *dI = tmp.upload(in, nin), *dO = tmp.alloc<float>(nout);
+    if (!s->envmap) return fail(s->ctx, B2_ERR_INVALID, "b2_envmap_probe: the scene has no environment map");
+    if (!in || !out || what < 0 || what > 2) return fail(s->ctx, B2_ERR_INVALID, "b2_envmap_probe: invalid argument");
     const Kernels kn = kernelsFor(s, parity_mode != 0);
-    kn.set.envmap_probe(kn.cfg, s->ds, what, n, dI, dO, ctx->stream);
-    CK(ctx, cudaStreamSynchronize(ctx->stream));
-    CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(out, dO, nout * sizeof(float), cudaMemcpyDeviceToHost));
-    return B2_OK;
+    return componentCall(s->ctx, "b2_envmap_probe", {{in, (what == 1 ? 9 : 3) * n}}, {{out, (what == 2 ? 1 : 3) * n}},
+                         [&](float *const *d) { kn.set.envmap_probe(kn.cfg, s->ds, what, n, d[0], d[1], s->ctx->stream); });
 }
 extern "C" int b2_texture_partials(b2_scene *s, uint64_t n, const float *pos_hit, int spp, int parity_mode, float *out) {
     NEED_COMMIT(s);
-    b2_ctx *ctx = s->ctx;
-    if (!pos_hit || !out || spp <= 0) return fail(ctx, B2_ERR_INVALID, "b2_texture_partials: invalid argument");
-    if (s->ds.nItems) return fail(ctx, B2_ERR_INVALID, "b2_texture_partials: instanced scenes are not supported by this probe");
-    CK(ctx, cudaSetDevice(ctx->device));
-    TmpDev tmp;
-    float *dI = tmp.upload(pos_hit, 6 * n), *dO = tmp.alloc<float>(6 * n);
+    if (!pos_hit || !out || spp <= 0) return fail(s->ctx, B2_ERR_INVALID, "b2_texture_partials: invalid argument");
+    if (s->ds.nItems) return fail(s->ctx, B2_ERR_INVALID, "b2_texture_partials: instanced scenes are not supported by this probe");
     const float diffScale = 1.0f / std::sqrt((float) spp);
     const Kernels kn = kernelsFor(s, parity_mode != 0);
-    kn.set.texture_probe(kn.cfg, s->ds, 1, 0, 0, diffScale, n, dI, dO, ctx->stream);
-    CK(ctx, cudaStreamSynchronize(ctx->stream));
-    CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(out, dO, 6 * n * sizeof(float), cudaMemcpyDeviceToHost));
-    return B2_OK;
+    return componentCall(s->ctx, "b2_texture_partials", {{pos_hit, 6 * n}}, {{out, 6 * n}},
+                         [&](float *const *d) { kn.set.texture_probe(kn.cfg, s->ds, 1, 0, 0, diffScale, n, d[0], d[1], s->ctx->stream); });
 }
 // One level of the MIP pyramid b2_scene_commit built (host data; RGB or luminance as given).  `out` may be NULL to query the size.
 extern "C" int b2_texture_level(b2_scene *s, int texture_id, int level, int *levels, int *width, int *height, float *out) {
@@ -1131,54 +1096,37 @@ extern "C" int b2_texture_level(b2_scene *s, int texture_id, int level, int *lev
 }
 extern "C" int b2_camera_rays(b2_scene *s, uint64_t n, const float *pos, int parity_mode, float *rays) {
     NEED_COMMIT(s);
-    b2_ctx *ctx = s->ctx;
-    CK(ctx, cudaSetDevice(ctx->device));
-    TmpDev tmp;
-    float *dP = tmp.upload(pos, 2 * n), *dR = tmp.alloc<float>(8 * n);
     const Kernels kn = kernelsFor(s, parity_mode != 0);
-    kn.set.camera_rays(kn.cfg, s->ds, n, dP, dR, ctx->stream);
-    CK(ctx, cudaStreamSynchronize(ctx->stream));
-    CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(rays, dR, 8 * n * sizeof(float), cudaMemcpyDeviceToHost));
-    return B2_OK;
+    return componentCall(s->ctx, "b2_camera_rays", {{pos, 2 * n}}, {{rays, 8 * n}},
+                         [&](float *const *d) { kn.set.camera_rays(kn.cfg, s->ds, n, d[0], d[1], s->ctx->stream); });
 }
 extern "C" int b2_sampler_stream(b2_scene *s, int sampler, uint64_t seed, int spp, int px, int py, int sample_idx, int ndim, float *out) {
     NEED_COMMIT(s);
-    b2_ctx *ctx = s->ctx;
-    CK(ctx, cudaSetDevice(ctx->device));
+    CK(s->ctx, cudaSetDevice(s->ctx->device));
     b2_render_params p;
     memset(&p, 0, sizeof(p));
     p.spp = spp; p.sampler = sampler; p.seed = seed; p.max_depth = -1; p.rr_depth = 5;
     DRender r;
-    int rc = fillRender(s, &p, r);
-    if (rc) return rc;
-    TmpDev tmp;
-    float *dO = tmp.alloc<float>(ndim);
-    parity::kernels.sampler_stream(s->ds, r, px, py, sample_idx, ndim, dO, ctx->stream);
-    CK(ctx, cudaStreamSynchronize(ctx->stream));
-    CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(out, dO, ndim * sizeof(float), cudaMemcpyDeviceToHost));
-    return B2_OK;
+    if (int rc = fillRender(s, &p, r)) return rc;
+    return componentCall(s->ctx, "b2_sampler_stream", {}, {{out, (size_t) ndim}},
+                         [&](float *const *d) { parity::kernels.sampler_stream(s->ds, r, px, py, sample_idx, ndim, d[0], s->ctx->stream); });
 }
 extern "C" int b2_splat(b2_ctx *ctx, int W, int H, int rfilter, float param, uint64_t n, const float *pos, const float *val, float *film) {
     if (!ctx || !pos || !val || !film || W <= 0 || H <= 0) return fail(ctx, B2_ERR_INVALID, "b2_splat: invalid argument");
-    CK(ctx, cudaSetDevice(ctx->device));
     DFilter f;
-    int rc = makeFilter(ctx, rfilter, param, f);
-    if (rc) return rc;
-    TmpDev tmp;
+    if (int rc = makeFilter(ctx, rfilter, param, f)) return rc;
+    CK(ctx, cudaSetDevice(ctx->device));
     const size_t nPix = (size_t) W * H;
-    float *dP = tmp.upload(pos, 2 * n), *dV = tmp.upload(val, 4 * n);
-    float4 *dRGBA = tmp.alloc<float4>(nPix);
-    float *dW = tmp.alloc<float>(nPix), *dOut = tmp.alloc<float>(5 * nPix);
-    cudaMemsetAsync(dRGBA, 0, nPix * sizeof(float4), ctx->stream);
-    cudaMemsetAsync(dW, 0, nPix * sizeof(float), ctx->stream);
+    DevBuf<float4> rgba;
+    DevBuf<float> w;
+    CK(ctx, rgba.alloc(nPix));
+    CK(ctx, w.alloc(nPix));
+    CK(ctx, cudaMemsetAsync(rgba.p, 0, nPix * sizeof(float4), ctx->stream));
+    CK(ctx, cudaMemsetAsync(w.p, 0, nPix * sizeof(float), ctx->stream));
     LaunchCfg cfg;
     cfg.numSMs = ctx->numSMs;
-    parity::kernels.splat(cfg, f, W, H, n, dP, dV, dRGBA, dW, ctx->stream);
-    parity::kernels.film_pack(cfg, dRGBA, dW, dOut, nPix, ctx->stream);
-    CK(ctx, cudaStreamSynchronize(ctx->stream));
-    CK(ctx, cudaGetLastError());
-    CK(ctx, cudaMemcpy(film, dOut, 5 * nPix * sizeof(float), cudaMemcpyDeviceToHost));
-    return B2_OK;
+    return componentCall(ctx, "b2_splat", {{pos, 2 * n}, {val, 4 * n}}, {{film, 5 * nPix}}, [&](float *const *d) {
+        parity::kernels.splat(cfg, f, W, H, n, d[0], d[1], rgba.p, w.p, ctx->stream);
+        parity::kernels.film_pack(cfg, rgba.p, w.p, d[2], nPix, ctx->stream);
+    });
 }

@@ -54,6 +54,10 @@ struct HostEmitter {
     bool env = false; // `constant` environment emitter (no parent shape)
 };
 
+// Stream rule: every upload and memset the library issues goes on the context stream (b2_ctx::stream), and a host read of device
+// memory comes after a synchronise of that stream.  The stream is non-blocking, so it does not wait for the legacy
+// default stream that a synchronous cudaMemcpy uses: a kernel on it is only ordered after copies queued on it.  A pageable source may
+// go out of scope as soon as cudaMemcpyAsync returns: the copy stages it first.
 template <typename T> struct DevBuf {
     T *p = nullptr;
     size_t n = 0;
@@ -61,6 +65,8 @@ template <typename T> struct DevBuf {
     void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
     // takes over a cudaMalloc'd array of `count` elements
     void adopt(T *q, size_t count) { release(); p = q; n = count; }
+    // gives the array up to the caller, who frees it
+    T *detach() { T *q = p; p = nullptr; n = 0; return q; }
     cudaError_t alloc(size_t count) {
         if (count == n && p) return cudaSuccess;
         release();
@@ -68,10 +74,10 @@ template <typename T> struct DevBuf {
         if (count == 0) return cudaSuccess;
         return cudaMalloc((void **) &p, count * sizeof(T));
     }
-    cudaError_t upload(const std::vector<T> &v) {
+    cudaError_t upload(const std::vector<T> &v, cudaStream_t st) {
         cudaError_t e = alloc(v.size());
         if (e != cudaSuccess || v.empty()) return e;
-        return cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
+        return cudaMemcpyAsync(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, st);
     }
 };
 

@@ -649,11 +649,25 @@ extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
     const Kernels kn = kernelsFor(s, parityMode);
     const KernelSet &K = kn.set;
     const LaunchCfg &cfg = kn.cfg;
-    uint32_t Q = p->pool_size > 0 ? (uint32_t) p->pool_size : (1u << 22); // 4M paths (~0.6 GB)
+    const bool volpath = p->integrator == B2_INTEGRATOR_VOLPATH;
+    int nClasses = 0, onlyClass = -1;
+    for (int c = 0; c < B2_NCLASS; ++c)
+        if (s->classPresent[c]) { ++nClasses; onlyClass = c == B2_NCLASS - 1 ? -1 : c; }
+    // more than one class: k_extend bins the hits by BSDF class and every class gets its own shading launch over its queue -- the four
+    // specialised instances, and the generic instance for the rest (null, twosided, dielectric, conductor, plastic); scenes with bitmap
+    // textures or an environment map use the TEX instances of the same classes (launch_shade)
+    bool sorted = nClasses > 1;
+    if (p->flags & 2) sorted = false;
+    // a shared-memory resident scene shaded by one instance: k_bounce_flat runs each path to its end (or its vertex budget) and k_generate
+    // drains the pool in slot order
+    const bool resident = !volpath && s->ds.rootCount && !sorted;
+    r.drainSlots = resident ? 1 : 0;
+    // 4M paths (~0.6 GB); also on the resident route, where Q only sets how much work one launch covers: 8 Mi and 16 Mi were slower
+    // at the Cornell headline (DESIGN.md section 6)
+    uint32_t Q = p->pool_size > 0 ? (uint32_t) p->pool_size : (1u << 22);
     Q = std::max<uint32_t>(Q, 1024u);
     Q = (uint32_t) std::min<uint64_t>(Q, std::max<uint64_t>(1024u, r.totalWork));
     Q = (Q + 255u) & ~255u;
-    const bool volpath = p->integrator == B2_INTEGRATOR_VOLPATH;
     rc = ensurePool(s, Q, volpath);
     if (rc) return rc;
     const size_t nPix = (size_t) s->W * s->H;
@@ -691,14 +705,6 @@ extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
     CK(ctx, cudaMemsetAsync(R.dFilmW.p, 0, nPix * sizeof(float), st));
     CK(ctx, cudaMemsetAsync(s->dCounters.p, 0, CTR_COUNT * sizeof(unsigned long long), st));
     CK(ctx, cudaMemsetAsync(R.pFlags.p, 0, (size_t) Q * sizeof(uint32_t), st));
-    int nClasses = 0, onlyClass = -1;
-    for (int c = 0; c < B2_NCLASS; ++c)
-        if (s->classPresent[c]) { ++nClasses; onlyClass = c == B2_NCLASS - 1 ? -1 : c; }
-    // more than one class: k_extend bins the hits by BSDF class and every class gets its own shading launch over its queue -- the four
-    // specialised instances, and the generic instance for the rest (null, twosided, dielectric, conductor, plastic); scenes with bitmap
-    // textures or an environment map use the TEX instances of the same classes (launch_shade)
-    bool sorted = nClasses > 1;
-    if (p->flags & 2) sorted = false;
     s->cancel.store(0);
     // every early return below leaves the stream idle and releases the events / the captured graph
     struct RenderGuard {
@@ -743,7 +749,7 @@ extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
             launchesPerIter = 3;
             return;
         }
-        if (s->ds.rootCount && !sorted) { // shared-memory resident scene, one shading instance: extend + shade + occluded in one launch
+        if (resident) { // shared-memory resident scene, one shading instance: extend + shade + occluded in one launch
             tick(2); K.bounce_flat(cfg, s->ds, s->pool, r, nClasses == 1 ? onlyClass : -1, st); tick(-1);
             launchesPerIter = 3;
             return;

@@ -12,6 +12,7 @@ struct LaunchCfg {
     int numSMs = 0;
     size_t traceSmem = 0;
     int gridExtend = 0, gridExtendSort = 0, gridOccluded = 0, gridTrace = 0, gridGenerate = 0, gridVolLockstep = 0;
+    int gridGenerateSlots = 0; // k_generate<SLOTS = true>: the slot-order drain of k_bounce_flat's route
     int gridShade[5] = {0, 0, 0, 0, 0};
     int gridShadeTex = 0; // k_shade<-1, TEX = true> (textured scenes)
     int gridShadeTexCls[4] = {0, 0, 0, 0}; // k_shade<c, TEX = true>: class-sorted dispatch of textured / environment-mapped scenes

@@ -260,6 +260,7 @@ struct DRender {
     uint64_t totalWork;      // W*H*(hi-lo)
     uint32_t roundSpp;       // samples every tile receives per round of the work enumeration (divides hi - lo; workItemPixel)
     uint32_t tilesX, tilesY; // whole 8x8 tiles of the film (W / 8, H / 8); the remaining strips are enumerated pixel by pixel
+    int32_t drainSlots;      // k_bounce_flat's route: k_generate drains the pool in slot order, no finished-path queue (b2_render)
     float4 *filmRGBA;        // H*W float4 accumulators (r, g, b, weight * alpha)
     float *filmW;            // H*W accumulators of weight * (1 - alpha): touched only by samples whose camera ray missed
     const uint64_t *lookupNib; // [2][13][16] nibble tables of sobol look_up for this render's m: [0] vdc (delta), [1] inv

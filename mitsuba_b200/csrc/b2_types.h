@@ -240,7 +240,10 @@ enum { CTR_DONE0 = 0, CTR_SHADOW = 1, CTR_CLASS0 = 2, /* 2..5 */ CTR_DONE1 = 6, 
        CTR_UNOCCLUDED = 18,
        CTR_TICKET_EXT = 19, CTR_TICKET_OCC = 20, // work tickets of the persistent traversal loops (zeroed by k_publish)
        CTR_CLASSG = 21,  // fifth class queue: hits on BSDFs without a specialised shading kernel (null, twosided, dielectric, conductor, plastic)
-       CTR_COUNT = 22 };
+       // set by k_publish: QUIET, no path alive and every work item handed out; IDLE, QUIET held at the previous iteration, so nothing is
+       // left to splat either and k_generate<SLOTS> / k_bounce_flat return at once (the host queues iterations ahead of the end it sees)
+       CTR_QUIET = 22, CTR_IDLE = 23,
+       CTR_COUNT = 24 };
 
 // progress ring in mapped pinned host memory, written by k_publish: {sequence = iteration + 1, live paths, next work item, -}
 #define B2_RING 64

@@ -100,7 +100,8 @@ typedef struct b2_medium_desc {
  * (src/samplers/sobol.cpp:86-102, independent.cpp:52-58), rfilters (src/rfilters/{box,gaussian}.cpp). */
 enum { B2_SAMPLER_SOBOL = 0, B2_SAMPLER_INDEPENDENT = 2 };
 enum { B2_RFILTER_BOX = 0, B2_RFILTER_GAUSSIAN = 1 };
-enum { B2_INTEGRATOR_PATH = 0 /* src/integrators/path/path.cpp */, B2_INTEGRATOR_VOLPATH = 1 /* src/integrators/path/volpath.cpp */ };
+enum { B2_INTEGRATOR_PATH = 0 /* src/integrators/path/path.cpp */, B2_INTEGRATOR_VOLPATH = 1 /* src/integrators/path/volpath.cpp */,
+       B2_INTEGRATOR_DIRECT = 2 /* src/integrators/direct/direct.cpp */ };
 typedef struct b2_render_params {
     int32_t spp;             /* sampleCount */
     int32_t sampler;         /* B2_SAMPLER_* (independent = counter-based stream, see DESIGN.md) */
@@ -123,8 +124,8 @@ typedef struct b2_render_params {
                                 bit5: collect per-pixel path diagnostics (b2_get_pixel_stats); bit6: per-sample event traces (b2_get_path_traces);
                                 bit8: force the throughput kernels (parity_mode 0 renders `path` scenes that contain a transmissive BSDF with the
                                 IEEE kernels: such scenes amplify ulp-level differences chaotically, DESIGN.md "parity") */
-    int32_t integrator;      /* B2_INTEGRATOR_* (<integrator type="path"|"volpath">) */
-    int32_t reserved;        /* must be 0 */
+    int32_t integrator;      /* B2_INTEGRATOR_* (<integrator type="path"|"volpath"|"direct">) */
+    int16_t emitter_samples, bsdf_samples; /* direct only (emitterSamples / bsdfSamples, direct.cpp:93-108): >= 0, not both 0 */
 } b2_render_params;
 
 /* Counters with the meaning of the reference's statistics (path.cpp:24,290-291; skdtree.cpp:46-47) plus

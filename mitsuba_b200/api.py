@@ -41,7 +41,7 @@ class b2_render_params(C.Structure):
                 ("rr_depth", C.c_int32), ("strict_normals", C.c_int32), ("hide_emitters", C.c_int32),
                 ("rfilter", C.c_int32), ("rfilter_param", C.c_float), ("sample_lo", C.c_int32), ("sample_hi", C.c_int32),
                 ("parity_mode", C.c_int32), ("pool_size", C.c_int32), ("film_on_device", C.c_int32), ("flags", C.c_int32),
-                ("integrator", C.c_int32), ("reserved", C.c_int32)]
+                ("integrator", C.c_int32), ("emitter_samples", C.c_int16), ("bsdf_samples", C.c_int16)]
 
 
 class b2_medium_desc(C.Structure):
@@ -51,7 +51,7 @@ class b2_medium_desc(C.Structure):
                 ("aabb_max", C.c_float * 3), ("density", C.POINTER(C.c_float))]
 
 
-INTEGRATORS = {"path": 0, "volpath": 1}
+INTEGRATORS = {"path": 0, "volpath": 1, "direct": 2}
 
 
 class b2_stats(C.Structure):
@@ -141,6 +141,11 @@ def make_params(rp: RenderParams, parity=False, pool_size=0, film_on_device=Fals
     p.sample_lo, p.sample_hi = rp.sample_lo, rp.sample_hi
     p.parity_mode, p.pool_size, p.film_on_device, p.flags = int(parity), pool_size, int(film_on_device), flags
     p.integrator = INTEGRATORS[getattr(rp, "integrator", "path")]
+    for name in ("emitter_samples", "bsdf_samples"):   # int16 fields: an out-of-range count must not wrap into a valid one
+        v = int(getattr(rp, name, 1))
+        if not -32768 <= v <= 32767:
+            raise B2Error(f"{name} out of range: {v}")
+        setattr(p, name, v)
     return p
 
 
@@ -150,7 +155,8 @@ def params_to_render_params(p: b2_render_params) -> RenderParams:
     return RenderParams(spp=p.spp, sampler=inv_s[p.sampler], seed=p.seed, max_depth=p.max_depth, rr_depth=p.rr_depth,
                         strict_normals=bool(p.strict_normals), hide_emitters=bool(p.hide_emitters), rfilter=inv_f[p.rfilter],
                         rfilter_param=p.rfilter_param, sample_lo=p.sample_lo, sample_hi=p.sample_hi,
-                        integrator={v: k for k, v in INTEGRATORS.items()}[p.integrator])
+                        integrator={v: k for k, v in INTEGRATORS.items()}[p.integrator],
+                        emitter_samples=p.emitter_samples, bsdf_samples=p.bsdf_samples)
 
 
 class Context:

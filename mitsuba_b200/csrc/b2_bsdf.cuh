@@ -366,7 +366,7 @@ template <int HINT> B2_DEV float leafPdf(const DMaterial &d, const BRec &r, bool
     }
 }
 
-template <int HINT> B2_DEV Spectrum leafSample(const DMaterial &d, BRec &r, float &pdfOut, float sx, float sy, PathSampler &smp) {
+template <int HINT, typename Smp = PathSampler> B2_DEV Spectrum leafSample(const DMaterial &d, BRec &r, float &pdfOut, float sx, float sy, Smp &smp) {
     const V3 R = (r.hasTex && (d.type == 0 || d.type == 1 || d.type == 7)) ? r.texR : ld3(d.reflectance); // diffuse reflectance, (rough)conductor specularReflectance
     const int type = (HINT >= 0 && HINT < 3) ? HINT : d.type;
     if (type == 4) { // null.cpp:65-76
@@ -538,7 +538,7 @@ template <int HINT> B2_DEV float bsdfPdf1(const DMaterial *mats, int id, const B
     return p * (1 - probSpecular);
 }
 
-template <int HINT> B2_DEV Spectrum bsdfSample1(const DMaterial *mats, int id, BRec &r, float &pdfOut, float sx, float sy, PathSampler &smp) {
+template <int HINT, typename Smp = PathSampler> B2_DEV Spectrum bsdfSample1(const DMaterial *mats, int id, BRec &r, float &pdfOut, float sx, float sy, Smp &smp) {
     const DMaterial &d = mats[id];
     if (HINT >= 0 && HINT < 3) return leafSample<HINT>(d, r, pdfOut, sx, sy, smp);
     if (HINT != 3 && d.type != 3) return leafSample<-1>(d, r, pdfOut, sx, sy, smp);
@@ -603,7 +603,7 @@ template <int HINT> B2_DEV float bsdfPdf(const DMaterial *mats, int id, const BR
     }
     return bsdfPdf1<HINT>(mats, id, r);
 }
-template <int HINT> B2_DEV Spectrum bsdfSample(const DMaterial *mats, int id, BRec &r, float &pdfOut, float sx, float sy, PathSampler &smp) {
+template <int HINT, typename Smp = PathSampler> B2_DEV Spectrum bsdfSample(const DMaterial *mats, int id, BRec &r, float &pdfOut, float sx, float sy, Smp &smp) {
     if (HINT < 0 && mats[id].type == 5) {
         bool flipped = false;
         if (cosTheta(r.wi) < 0) { r.wi.z *= -1; flipped = true; }

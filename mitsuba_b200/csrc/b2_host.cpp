@@ -539,7 +539,17 @@ static int fillRender(b2_scene *s, const b2_render_params *p, DRender &r) {
     r.spp = p->spp; r.sampler = p->sampler;
     r.maxDepth = p->max_depth; r.rrDepth = p->rr_depth; r.strictNormals = p->strict_normals; r.hideEmitters = p->hide_emitters;
     r.sampleLo = p->sample_lo; r.sampleHi = p->sample_hi > 0 ? p->sample_hi : p->spp;
-    if (p->integrator != B2_INTEGRATOR_PATH && p->integrator != B2_INTEGRATOR_VOLPATH) return fail(ctx, B2_ERR_INVALID, "unknown integrator");
+    if (p->integrator != B2_INTEGRATOR_PATH && p->integrator != B2_INTEGRATOR_VOLPATH && p->integrator != B2_INTEGRATOR_DIRECT)
+        return fail(ctx, B2_ERR_INVALID, "unknown integrator");
+    if (p->integrator == B2_INTEGRATOR_DIRECT) { // direct.cpp:93-108
+        if (p->emitter_samples < 0 || p->bsdf_samples < 0) return fail(ctx, B2_ERR_INVALID, "direct: 'emitterSamples' and 'bsdfSamples' must not be negative");
+        if (p->emitter_samples + p->bsdf_samples == 0) return fail(ctx, B2_ERR_INVALID, "direct: 'emitterSamples' + 'bsdfSamples' must be positive");
+        // the index of an array entry, s * count + k, is a 32-bit sample index of the pixel (sobol.cpp:190)
+        if ((uint64_t) p->spp * (uint64_t) std::max(p->emitter_samples, p->bsdf_samples) >= (1ull << 32))
+            return fail(ctx, B2_ERR_INVALID, "direct: sampleCount x max(emitterSamples, bsdfSamples) must be below 2^32");
+        if (p->flags & (32 | 64)) return fail(ctx, B2_ERR_INVALID, "direct: per-path diagnostics (flags bit5 / bit6) have no meaning without paths");
+        r.emitterSamples = p->emitter_samples; r.bsdfSamples = p->bsdf_samples;
+    }
     if (p->integrator == B2_INTEGRATOR_VOLPATH && s->ds.nItems) return fail(ctx, B2_ERR_INVALID, "volpath with instanced geometry is not supported");
     if (p->integrator == B2_INTEGRATOR_VOLPATH && s->ds.nTextures) return fail(ctx, B2_ERR_INVALID, "volpath with bitmap textures is not supported");
     r.integrator = p->integrator;
@@ -572,7 +582,11 @@ static int fillRender(b2_scene *s, const b2_render_params *p, DRender &r) {
     r.totalWork = (uint64_t) s->W * (uint64_t) s->H * (uint64_t) (r.sampleHi - r.sampleLo);
     // nibble tables of sobol::look_up for this m (sobolseq.h:104-133) and the nibble counts that cover the indices
     auto bitsOf = [](uint64_t v) { uint32_t b = 0; while (v) { ++b; v >>= 1; } return b; };
-    const uint32_t frameBits = std::max(1u, bitsOf((uint64_t) r.sampleHi - 1));
+    // `direct` with sample arrays also looks up the pixel's points s * n + k below spp * n (sobol.cpp:190)
+    uint64_t maxFrame = (uint64_t) r.sampleHi - 1;
+    if (p->integrator == B2_INTEGRATOR_DIRECT && std::max(r.emitterSamples, r.bsdfSamples) > 1)
+        maxFrame = (uint64_t) p->spp * (uint64_t) std::max(r.emitterSamples, r.bsdfSamples) - 1;
+    const uint32_t frameBits = std::max(1u, bitsOf(maxFrame));
     r.frameNibbles = (frameBits + 3) / 4;
     r.bNibbles = (2 * r.logRes + 3) / 4;
     const uint32_t indexBits = (p->sampler == B2_SAMPLER_SOBOL && r.logRes > 1) ? frameBits + 2 * r.logRes : frameBits;
@@ -622,6 +636,73 @@ static int ensurePool(b2_scene *s, uint32_t Q, bool vol) {
     return B2_OK;
 }
 
+// `direct`: k_direct over the work items in slices of whole samples of the film, so that b2_cancel is honoured between launches; no
+// path pool.  Counters as for `path` except path_length_sum (direct keeps no such statistic).
+static int renderDirect(b2_scene *s, const b2_render_params *p, const DRender &r, const DFilter &filt, const Kernels &kn, float *film) {
+    b2_ctx *ctx = s->ctx;
+    RenderStore &R = *ctx->store;
+    cudaStream_t st = ctx->stream;
+    const size_t nPix = (size_t) s->W * s->H;
+    CK(ctx, R.dFilmRGBA.alloc(nPix));
+    CK(ctx, R.dFilmW.alloc(nPix));
+    DRender rr = r;
+    rr.filmRGBA = R.dFilmRGBA.p; rr.filmW = R.dFilmW.p;
+    CK(ctx, cudaMemsetAsync(R.dFilmRGBA.p, 0, nPix * sizeof(float4), st));
+    CK(ctx, cudaMemsetAsync(R.dFilmW.p, 0, nPix * sizeof(float), st));
+    CK(ctx, cudaMemsetAsync(s->dCounters.p, 0, CTR_COUNT * sizeof(unsigned long long), st));
+    s->cancel.store(0);
+    struct Guard {
+        cudaStream_t st;
+        cudaEvent_t a = nullptr, b = nullptr;
+        ~Guard() {
+            cudaStreamSynchronize(st);
+            if (a) cudaEventDestroy(a);
+            if (b) cudaEventDestroy(b);
+        }
+    } guard{st};
+    CK(ctx, cudaEventCreate(&guard.a));
+    CK(ctx, cudaEventCreate(&guard.b));
+    CK(ctx, cudaEventRecord(guard.a, st));
+    // a slice: enough whole samples of the film for ~16M items (a few ms on the flat route), at least one sample; the cancel flag is
+    // read before each launch
+    const uint64_t perSample = (uint64_t) nPix, nS = (uint64_t) (r.sampleHi - r.sampleLo);
+    const uint64_t slice = perSample * std::max<uint64_t>(1, std::min<uint64_t>(nS, (16ull << 20) / std::max<uint64_t>(1, perSample)));
+    uint64_t launches = 0;
+    int status = B2_OK;
+    for (uint64_t b = 0; b < r.totalWork; b += slice) {
+        if (s->cancel.load()) { status = B2_ERR_CANCELLED; break; }
+        if (launches >= 2) cudaStreamSynchronize(st); // from the third slice on, the host waits for the queued ones: a cancel waits for at most two slices, not for the render
+        kn.set.direct(kn.cfg, s->ds, rr, filt, s->dCounters.p, b, std::min(r.totalWork, b + slice), st);
+        ++launches;
+    }
+    CK(ctx, cudaGetLastError());
+    CK(ctx, cudaEventRecord(guard.b, st));
+    if (status == B2_OK) {
+        float *dOut = film;
+        if (!p->film_on_device) {
+            CK(ctx, R.dFilmOut.alloc(nPix * 5));
+            dOut = R.dFilmOut.p;
+        }
+        kn.set.film_pack(kn.cfg, R.dFilmRGBA.p, R.dFilmW.p, dOut, nPix, st);
+        if (!p->film_on_device) CK(ctx, cudaMemcpyAsync(film, dOut, nPix * 5 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    }
+    CK(ctx, cudaStreamSynchronize(st));
+    CK(ctx, cudaGetLastError());
+    std::vector<unsigned long long> ctr(CTR_COUNT);
+    CK(ctx, cudaMemcpy(ctr.data(), s->dCounters.p, CTR_COUNT * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, guard.a, guard.b);
+    b2_stats &t = s->stats;
+    t.ms_generate = t.ms_extend = t.ms_shade = t.ms_occluded = 0;
+    t.n_generate = t.n_extend = t.n_shade = t.n_occluded = 0;
+    t.pool_size = 0;
+    t.unoccluded_shadow_rays = ctr[CTR_UNOCCLUDED];
+    t.samples = ctr[CTR_SAMPLES]; t.rays = ctr[CTR_RAYS]; t.shadow_rays = ctr[CTR_SHADOWRAYS]; t.path_length_sum = 0;
+    t.bad_samples = ctr[CTR_BAD]; t.dim_overflow = ctr[CTR_DIMOVF]; t.iterations = launches; t.kernel_launches = launches + 1;
+    t.ms_total = ms;
+    return status;
+}
+
 extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
     if (!s || !p || !film) return fail(s ? s->ctx : nullptr, B2_ERR_INVALID, "b2_render: null argument");
     b2_ctx *ctx = s->ctx;
@@ -649,6 +730,7 @@ extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
     const Kernels kn = kernelsFor(s, parityMode);
     const KernelSet &K = kn.set;
     const LaunchCfg &cfg = kn.cfg;
+    if (p->integrator == B2_INTEGRATOR_DIRECT) return renderDirect(s, p, r, filt, kn, film);
     const bool volpath = p->integrator == B2_INTEGRATOR_VOLPATH;
     int nClasses = 0, onlyClass = -1;
     for (int c = 0; c < B2_NCLASS; ++c)

@@ -20,6 +20,9 @@ struct LaunchCfg {
     size_t flatSmem = 0;
     int gridExtendFlatSort = 0, gridOccludedFlat = 0;
     int gridBounceFlat[2][5] = {{0, 0, 0, 0, 0}, {0, 0, 0, 0, 0}};
+    // k_direct[TEX][walk]: walk 0 flat leaf, 1 binary BVH, 2 instances; its shared memory for the scene's walk
+    size_t directSmem = 0;
+    int gridDirect[2][3] = {{0, 0, 0}, {0, 0, 0}};
 };
 
 struct KernelSet {
@@ -48,6 +51,9 @@ struct KernelSet {
     void (*sampler_stream)(const DScene &, const DRender &, int px, int py, int sampleIdx, int ndim, float *out, cudaStream_t);
     void (*splat)(const LaunchCfg &, const DFilter &, int W, int H, uint64_t n, const float *pos, const float *val, float4 *rgba, float *wgt,
                   cudaStream_t);
+    // `direct`: work items [begin, end) of the render (camera ray to splat in one thread each); counters: CTR_* of the scene
+    void (*direct)(const LaunchCfg &, const DScene &, const DRender &, const DFilter &, unsigned long long *counters, uint64_t begin, uint64_t end,
+                   cudaStream_t);
 };
 
 namespace parity { extern const KernelSet kernels; }

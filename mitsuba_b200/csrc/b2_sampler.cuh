@@ -126,4 +126,32 @@ struct PathSampler {
     }
 };
 
+// The sampler of the `direct` integrator: the regular dimensions of a PathSampler that skip the range [5, arrayEnd) its 2-D sample
+// arrays occupy (sobol.cpp:218-238), and the array entries themselves.  Its own type, so that PathSampler and the kernels that use it
+// are compiled as before.  arrayEnd = 5 + 2 * (number of arrays) for Sobol' (with no array the range is empty and only next2D's jump
+// from dimension 4 to 5 remains, as in PathSampler); the counter stream skips only when there are arrays, and its arrays fill the
+// range entry by entry (DESIGN.md "direct").
+struct ArraySampler {
+    PathSampler p;
+    uint32_t arrayEnd;
+    bool skip;
+    B2_DEV float next1D() {
+        if (skip && p.dim >= 5u && p.dim < arrayEnd) p.dim = arrayEnd; // sobol.cpp:220-221
+        return p.next1D();
+    }
+    B2_DEV void next2D(float &a, float &b) {
+        if (skip && p.dim + 1u >= 5u && p.dim < arrayEnd) p.dim = arrayEnd; // sobol.cpp:234-235
+        if (p.kind == 0 && p.dim + 1 >= 1024u) { p.overflow = true; p.dim = 1022u; }
+        a = p.next1D();
+        b = p.next1D();
+    }
+};
+
+// word d of the counter stream of key (see PathSampler::next1D)
+B2_DEV float counterAt(uint32_t key, uint32_t seedHi, uint32_t d) {
+    const uint64_t r = sampleTEA(key, (d >> 1) ^ seedHi, 8);
+    const uint32_t w = (d & 1u) ? (uint32_t) (r >> 32) : (uint32_t) r;
+    return __uint_as_float((w >> 9) | 0x3f800000u) - 1.0f;
+}
+
 } // namespace b2

@@ -274,6 +274,7 @@ struct DRender {
     unsigned long long *pathTrace;  // null unless per-sample event traces were requested (flags bit6): [pixel * nS + s] gets one event byte per bounce
     unsigned long long *stampStart; // null unless per-launch timing was requested (b2_render_params.flags bit2)
     unsigned long long *stampEnd;
+    int32_t emitterSamples, bsdfSamples; // direct: sample counts of the two strategies (direct.cpp:93-108)
 };
 
 } // namespace b2

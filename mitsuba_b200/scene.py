@@ -379,7 +379,9 @@ class RenderParams:
     hide_emitters: bool = False
     rfilter: str = "gaussian"           # film.cpp:89-95 default
     rfilter_param: float = 0.5          # box: radius; gaussian: stddev
-    integrator: str = "path"            # "path" (path.cpp) | "volpath" (volpath.cpp)
+    integrator: str = "path"            # "path" (path.cpp) | "volpath" (volpath.cpp) | "direct" (direct.cpp)
+    emitter_samples: int = 1            # direct only: emitterSamples / bsdfSamples (direct.cpp:93-108)
+    bsdf_samples: int = 1
     sample_lo: int = 0                  # shard: sample indices [lo,hi) of every pixel
     sample_hi: int = 0                  # 0 -> spp
 

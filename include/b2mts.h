@@ -120,7 +120,7 @@ typedef struct b2_render_params {
     int32_t film_on_device;  /* 1: `film` of b2_render is a device pointer on the context's device */
     int32_t flags;           /* bit1: force unsorted shading (default: material-sorted when > 1 BSDF class);
                                 bit2: per-launch device time stamps (fills b2_stats.ms_*); bit3: plain launches + CUDA events
-                                instead of the CUDA graph; bit4: fuse the ray casts into generate/shade for tiny scenes (experiment, slower);
+                                instead of the CUDA graph;
                                 bit5: collect per-pixel path diagnostics (b2_get_pixel_stats); bit6: per-sample event traces (b2_get_path_traces);
                                 bit8: force the throughput kernels (parity_mode 0 renders `path` scenes that contain a transmissive BSDF with the
                                 IEEE kernels: such scenes amplify ulp-level differences chaotically, DESIGN.md "parity") */

@@ -612,7 +612,8 @@ static int fillRender(b2_scene *s, const b2_render_params *p, DRender &r) {
     return B2_OK;
 }
 
-static int ensurePool(b2_scene *s, uint32_t Q, bool vol) {
+// Points the scene's DPool and `r` at a pool of Q empty slots and at a cleared progress ring.
+static int ensurePool(b2_scene *s, uint32_t Q, bool vol, DRender &r) {
     b2_ctx *ctx = s->ctx;
     RenderStore &R = *ctx->store;
     if (R.capacity != Q) {
@@ -633,138 +634,53 @@ static int ensurePool(b2_scene *s, uint32_t Q, bool vol) {
     p.counters = s->dCounters.p;
     p.vol = R.pVol.p;
     p.inst = R.pInst.p;
-    return B2_OK;
-}
-
-// `direct`: k_direct over the work items in slices of whole samples of the film, so that b2_cancel is honoured between launches; no
-// path pool.  Counters as for `path` except path_length_sum (direct keeps no such statistic).
-static int renderDirect(b2_scene *s, const b2_render_params *p, const DRender &r, const DFilter &filt, const Kernels &kn, float *film) {
-    b2_ctx *ctx = s->ctx;
-    RenderStore &R = *ctx->store;
-    cudaStream_t st = ctx->stream;
-    const size_t nPix = (size_t) s->W * s->H;
-    CK(ctx, R.dFilmRGBA.alloc(nPix));
-    CK(ctx, R.dFilmW.alloc(nPix));
-    DRender rr = r;
-    rr.filmRGBA = R.dFilmRGBA.p; rr.filmW = R.dFilmW.p;
-    CK(ctx, cudaMemsetAsync(R.dFilmRGBA.p, 0, nPix * sizeof(float4), st));
-    CK(ctx, cudaMemsetAsync(R.dFilmW.p, 0, nPix * sizeof(float), st));
-    CK(ctx, cudaMemsetAsync(s->dCounters.p, 0, CTR_COUNT * sizeof(unsigned long long), st));
-    s->cancel.store(0);
-    struct Guard {
-        cudaStream_t st;
-        cudaEvent_t a = nullptr, b = nullptr;
-        ~Guard() {
-            cudaStreamSynchronize(st);
-            if (a) cudaEventDestroy(a);
-            if (b) cudaEventDestroy(b);
-        }
-    } guard{st};
-    CK(ctx, cudaEventCreate(&guard.a));
-    CK(ctx, cudaEventCreate(&guard.b));
-    CK(ctx, cudaEventRecord(guard.a, st));
-    // a slice: enough whole samples of the film for ~16M items (a few ms on the flat route), at least one sample; the cancel flag is
-    // read before each launch
-    const uint64_t perSample = (uint64_t) nPix, nS = (uint64_t) (r.sampleHi - r.sampleLo);
-    const uint64_t slice = perSample * std::max<uint64_t>(1, std::min<uint64_t>(nS, (16ull << 20) / std::max<uint64_t>(1, perSample)));
-    uint64_t launches = 0;
-    int status = B2_OK;
-    for (uint64_t b = 0; b < r.totalWork; b += slice) {
-        if (s->cancel.load()) { status = B2_ERR_CANCELLED; break; }
-        if (launches >= 2) cudaStreamSynchronize(st); // from the third slice on, the host waits for the queued ones: a cancel waits for at most two slices, not for the render
-        kn.set.direct(kn.cfg, s->ds, rr, filt, s->dCounters.p, b, std::min(r.totalWork, b + slice), st);
-        ++launches;
-    }
-    CK(ctx, cudaGetLastError());
-    CK(ctx, cudaEventRecord(guard.b, st));
-    if (status == B2_OK) {
-        float *dOut = film;
-        if (!p->film_on_device) {
-            CK(ctx, R.dFilmOut.alloc(nPix * 5));
-            dOut = R.dFilmOut.p;
-        }
-        kn.set.film_pack(kn.cfg, R.dFilmRGBA.p, R.dFilmW.p, dOut, nPix, st);
-        if (!p->film_on_device) CK(ctx, cudaMemcpyAsync(film, dOut, nPix * 5 * sizeof(float), cudaMemcpyDeviceToHost, st));
-    }
-    CK(ctx, cudaStreamSynchronize(st));
-    CK(ctx, cudaGetLastError());
-    std::vector<unsigned long long> ctr(CTR_COUNT);
-    CK(ctx, cudaMemcpy(ctr.data(), s->dCounters.p, CTR_COUNT * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, guard.a, guard.b);
-    b2_stats &t = s->stats;
-    t.ms_generate = t.ms_extend = t.ms_shade = t.ms_occluded = 0;
-    t.n_generate = t.n_extend = t.n_shade = t.n_occluded = 0;
-    t.pool_size = 0;
-    t.unoccluded_shadow_rays = ctr[CTR_UNOCCLUDED];
-    t.samples = ctr[CTR_SAMPLES]; t.rays = ctr[CTR_RAYS]; t.shadow_rays = ctr[CTR_SHADOWRAYS]; t.path_length_sum = 0;
-    t.bad_samples = ctr[CTR_BAD]; t.dim_overflow = ctr[CTR_DIMOVF]; t.iterations = launches; t.kernel_launches = launches + 1;
-    t.ms_total = ms;
-    return status;
-}
-
-extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
-    if (!s || !p || !film) return fail(s ? s->ctx : nullptr, B2_ERR_INVALID, "b2_render: null argument");
-    b2_ctx *ctx = s->ctx;
-    if (!s->committed) return fail(ctx, B2_ERR_INVALID, "b2_render: scene not committed");
-    CK(ctx, cudaSetDevice(ctx->device));
-    RenderStore &R = *ctx->store;
-    std::lock_guard<std::mutex> renderLock(R.renderMutex);
-    cudaStream_t st = ctx->stream;
-    DRender r;
-    int rc = fillRender(s, p, r);
-    if (rc) return rc;
-    DFilter filt;
-    rc = makeFilter(ctx, p->rfilter, p->rfilter_param, filt);
-    if (rc) return rc;
-    // Which kernel set renders?  parity_mode 1: the IEEE build (-fmad=false, accurate division / sqrt / sincos, TriAccel).  parity_mode 0: the
-    // throughput build -- EXCEPT for `path` renders of scenes with a transmissive BSDF.  A path that bounces inside a glass ball amplifies
-    // ulp-level differences chaotically: under FMA contraction alone a few in 1e5 of such paths leave the reference's path (different hit,
-    // other lobe, other ending -- not fast-math, not the plane-form triangle test), each an unrelated sample of a heavy-tailed estimator,
-    // i.e. above 1e-3 relative L2 at 1024^2 @ 512 spp whatever else the kernels do.  Shading such scenes
-    // with the IEEE kernels and keeping only the traversal fast ("hybrid", tried: exact TriAccel (t,u,v) of the winning triangle) removes
-    // a third of the flips -- the fast traversal still picks the neighbouring triangle at shared edges -- so those scenes get the IEEE
-    // build as a whole (BVH traversal dominates BASELINE config 3, so the IEEE shading costs little there).  flags bit8 forces the throughput kernels.
-    const bool autoIeee = s->hasTransmission && p->integrator == B2_INTEGRATOR_PATH && !(p->flags & 256);
-    const bool parityMode = p->parity_mode != 0 || autoIeee;
-    const Kernels kn = kernelsFor(s, parityMode);
-    const KernelSet &K = kn.set;
-    const LaunchCfg &cfg = kn.cfg;
-    if (p->integrator == B2_INTEGRATOR_DIRECT) return renderDirect(s, p, r, filt, kn, film);
-    const bool volpath = p->integrator == B2_INTEGRATOR_VOLPATH;
-    int nClasses = 0, onlyClass = -1;
-    for (int c = 0; c < B2_NCLASS; ++c)
-        if (s->classPresent[c]) { ++nClasses; onlyClass = c == B2_NCLASS - 1 ? -1 : c; }
-    // more than one class: k_extend bins the hits by BSDF class and every class gets its own shading launch over its queue -- the four
-    // specialised instances, and the generic instance for the rest (null, twosided, dielectric, conductor, plastic); scenes with bitmap
-    // textures or an environment map use the TEX instances of the same classes (launch_shade)
-    bool sorted = nClasses > 1;
-    if (p->flags & 2) sorted = false;
-    // a shared-memory resident scene shaded by one instance: k_bounce_flat runs each path to its end (or its vertex budget) and k_generate
-    // drains the pool in slot order
-    const bool resident = !volpath && s->ds.rootCount && !sorted;
-    r.drainSlots = resident ? 1 : 0;
-    // 4M paths (~0.6 GB); also on the resident route, where Q only sets how much work one launch covers: 8 Mi and 16 Mi were slower
-    // at the Cornell headline (DESIGN.md section 6)
-    uint32_t Q = p->pool_size > 0 ? (uint32_t) p->pool_size : (1u << 22);
-    Q = std::max<uint32_t>(Q, 1024u);
-    Q = (uint32_t) std::min<uint64_t>(Q, std::max<uint64_t>(1024u, r.totalWork));
-    Q = (Q + 255u) & ~255u;
-    rc = ensurePool(s, Q, volpath);
-    if (rc) return rc;
-    const size_t nPix = (size_t) s->W * s->H;
-    CK(ctx, R.dFilmRGBA.alloc(nPix));
-    CK(ctx, R.dFilmW.alloc(nPix));
-    r.filmRGBA = R.dFilmRGBA.p; r.filmW = R.dFilmW.p;
+    CK(ctx, cudaMemsetAsync(R.pFlags.p, 0, (size_t) Q * sizeof(uint32_t), ctx->stream));
     if (!R.hRing) {
         CK(ctx, cudaHostAlloc((void **) &R.hRing, sizeof(unsigned long long) * 4 * B2_RING, cudaHostAllocMapped));
         CK(ctx, cudaHostGetDevicePointer((void **) &R.dRing, R.hRing, 0));
     }
     memset(R.hRing, 0, sizeof(unsigned long long) * 4 * B2_RING);
     r.ring = R.dRing;
-    const bool timing = (p->flags & 4) != 0;      // per-launch device time stamps (%globaltimer inside the kernels)
-    const bool useEvents = (p->flags & 8) != 0;   // no graph: plain launches bracketed by CUDA events (cross-check path)
-    if (timing) {
+    return B2_OK;
+}
+
+// The route of a `path` / `volpath` render: which kernels one iteration launches, and how many paths are in flight.
+struct Route {
+    bool volpath, sorted, resident;
+    int shadeClass; // unsorted shading: the instance of the scene's one BSDF class, -1 for the generic one
+    uint32_t Q;
+};
+static Route chooseRoute(const b2_scene *s, const b2_render_params *p, DRender &r) {
+    Route w;
+    w.volpath = p->integrator == B2_INTEGRATOR_VOLPATH;
+    int nClasses = 0, onlyClass = -1;
+    for (int c = 0; c < B2_NCLASS; ++c)
+        if (s->classPresent[c]) { ++nClasses; onlyClass = c == B2_NCLASS - 1 ? -1 : c; }
+    w.shadeClass = nClasses == 1 ? onlyClass : -1;
+    // more than one class: k_extend bins the hits by BSDF class and every class gets its own shading launch over its queue -- the four
+    // specialised instances, and the generic instance for the rest (null, twosided, dielectric, conductor, plastic); scenes with bitmap
+    // textures or an environment map use the TEX instances of the same classes (launch_shade)
+    w.sorted = nClasses > 1 && !(p->flags & 2);
+    // a shared-memory resident scene shaded by one instance: k_bounce_flat runs each path to its end (or its vertex budget) and k_generate
+    // drains the pool in slot order
+    w.resident = !w.volpath && s->ds.rootCount && !w.sorted;
+    r.drainSlots = w.resident ? 1 : 0;
+    // 4M paths (~0.6 GB); also on the resident route, where Q only sets how much work one launch covers: 8 Mi and 16 Mi were slower
+    // at the Cornell headline (DESIGN.md section 6)
+    uint32_t Q = p->pool_size > 0 ? (uint32_t) p->pool_size : (1u << 22);
+    Q = std::max<uint32_t>(Q, 1024u);
+    Q = (uint32_t) std::min<uint64_t>(Q, std::max<uint64_t>(1024u, r.totalWork));
+    w.Q = (Q + 255u) & ~255u;
+    return w;
+}
+
+// The cleared diagnostic buffers of a `path` / `volpath` render: time stamps (flags bit2), pixel statistics (bit5), path traces (bit6)
+static int diagnosticBuffers(b2_scene *s, const b2_render_params *p, DRender &r) {
+    b2_ctx *ctx = s->ctx;
+    RenderStore &R = *ctx->store;
+    const cudaStream_t st = ctx->stream;
+    const size_t nPix = (size_t) s->W * s->H;
+    if (p->flags & 4) { // per-launch device time stamps (%globaltimer inside the kernels)
         CK(ctx, R.dStampStart.alloc((size_t) B2_MAX_STAMPS * 4));
         CK(ctx, R.dStampEnd.alloc((size_t) B2_MAX_STAMPS * 4));
         CK(ctx, cudaMemsetAsync(R.dStampStart.p, 0xFF, (size_t) B2_MAX_STAMPS * 4 * 8, st));
@@ -783,136 +699,187 @@ extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
         CK(ctx, cudaMemsetAsync(R.dPathTrace.p, 0, nTr * sizeof(unsigned long long), st));
         r.pathTrace = R.dPathTrace.p;
     }
-    CK(ctx, cudaMemsetAsync(R.dFilmRGBA.p, 0, nPix * sizeof(float4), st));
-    CK(ctx, cudaMemsetAsync(R.dFilmW.p, 0, nPix * sizeof(float), st));
-    CK(ctx, cudaMemsetAsync(s->dCounters.p, 0, CTR_COUNT * sizeof(unsigned long long), st));
-    CK(ctx, cudaMemsetAsync(R.pFlags.p, 0, (size_t) Q * sizeof(uint32_t), st));
-    s->cancel.store(0);
-    // every early return below leaves the stream idle and releases the events / the captured graph
-    struct RenderGuard {
-        cudaStream_t st;
-        cudaEvent_t a = nullptr, b = nullptr;
-        cudaGraph_t *graph = nullptr;
-        cudaGraphExec_t *exec = nullptr;
-        ~RenderGuard() {
-            cudaStreamSynchronize(st);
-            if (exec && *exec) cudaGraphExecDestroy(*exec);
-            if (graph && *graph) cudaGraphDestroy(*graph);
-            if (a) cudaEventDestroy(a);
-            if (b) cudaEventDestroy(b);
-        }
-    } guard{st};
-    cudaEvent_t evStart, evStop;
-    CK(ctx, cudaEventCreate(&evStart));
-    guard.a = evStart;
-    CK(ctx, cudaEventCreate(&evStop));
-    guard.b = evStop;
-    CK(ctx, cudaEventRecord(evStart, st));
-    uint64_t iter = 0, checked = 0, launches = 0;
-    bool finished = false;
-    int status = B2_OK;
-    std::vector<std::pair<int, size_t>> timed; // (stage, index of the start event) -- events path only
-    size_t evUsed = 0;
-    auto tick = [&](int stage) {
-        if (!useEvents) return;
-        if (evUsed == s->timingEvents.size()) { cudaEvent_t e; cudaEventCreate(&e); s->timingEvents.push_back(e); }
-        cudaEventRecord(s->timingEvents[evUsed], st);
-        if (stage >= 0) timed.emplace_back(stage, evUsed);
-        ++evUsed;
-    };
-    int launchesPerIter = 0;
-    // one iteration = generate (+publish) -> extend -> shade (per material class) -> occluded; flat scenes shaded by one launch:
-    // generate (+publish) -> bounce
-    auto enqueueIteration = [&]() {
-        launchesPerIter = 0;
-        tick(0); K.generate(cfg, s->ds, s->pool, r, filt, st); tick(-1);
-        if (volpath) { // volpath: every ray of an iteration is cast inline by k_volstep_lockstep
-            tick(2); K.volstep(cfg, s->ds, s->pool, r, st); tick(-1);
-            launchesPerIter = 3;
-            return;
-        }
-        if (resident) { // shared-memory resident scene, one shading instance: extend + shade + occluded in one launch
-            tick(2); K.bounce_flat(cfg, s->ds, s->pool, r, nClasses == 1 ? onlyClass : -1, st); tick(-1);
-            launchesPerIter = 3;
-            return;
-        }
-        tick(1); K.extend(cfg, s->ds, s->pool, r, sorted, st); tick(-1); ++launchesPerIter;
-        tick(2);
-        if (sorted) {
-            for (int c = 0; c < B2_NCLASS; ++c)
-                if (s->classPresent[c]) { K.shade(cfg, s->ds, s->pool, r, c, true, st); ++launchesPerIter; }
-        } else {
-            K.shade(cfg, s->ds, s->pool, r, nClasses == 1 ? onlyClass : -1, false, st);
-            ++launchesPerIter;
-        }
-        tick(-1);
-        tick(3); K.occluded(cfg, s->ds, s->pool, r, st); tick(-1); ++launchesPerIter;
-        launchesPerIter += 2;
-    };
+    return B2_OK;
+}
+
+// CUDA events around the stages of every iteration (flags bit3), reused from render to render: tick(stage) records the start of a stage,
+// tick(-1) its end
+struct StageEvents {
+    b2_scene *s;
+    bool on;
+    std::vector<std::pair<int, size_t>> timed; // (stage, index of the start event)
+    size_t used = 0;
+    void tick(int stage) {
+        if (!on) return;
+        if (used == s->timingEvents.size()) { cudaEvent_t e; cudaEventCreate(&e); s->timingEvents.push_back(e); }
+        cudaEventRecord(s->timingEvents[used], s->ctx->stream);
+        if (stage >= 0) timed.emplace_back(stage, used);
+        ++used;
+    }
+};
+
+// Queues one iteration and returns its number of kernel launches.  One iteration = generate (+publish) -> extend -> shade (per material
+// class) -> occluded; flat scenes shaded by one launch: generate (+publish) -> bounce
+static int enqueueIteration(b2_scene *s, const Route &w, const DRender &r, const DFilter &filt, const Kernels &kn, StageEvents &ev) {
+    const KernelSet &K = kn.set;
+    const LaunchCfg &cfg = kn.cfg;
+    const cudaStream_t st = s->ctx->stream;
+    ev.tick(0); K.generate(cfg, s->ds, s->pool, r, filt, st); ev.tick(-1);
+    if (w.volpath) { // volpath: every ray of an iteration is cast inline by k_volstep_lockstep
+        ev.tick(2); K.volstep(cfg, s->ds, s->pool, r, st); ev.tick(-1);
+        return 3;
+    }
+    if (w.resident) { // shared-memory resident scene, one shading instance: extend + shade + occluded in one launch
+        ev.tick(2); K.bounce_flat(cfg, s->ds, s->pool, r, w.shadeClass, st); ev.tick(-1);
+        return 3;
+    }
+    int launches = 0;
+    ev.tick(1); K.extend(cfg, s->ds, s->pool, r, w.sorted, st); ev.tick(-1); ++launches;
+    ev.tick(2);
+    if (w.sorted) {
+        for (int c = 0; c < B2_NCLASS; ++c)
+            if (s->classPresent[c]) { K.shade(cfg, s->ds, s->pool, r, c, true, st); ++launches; }
+    } else {
+        K.shade(cfg, s->ds, s->pool, r, w.shadeClass, false, st);
+        ++launches;
+    }
+    ev.tick(-1);
+    ev.tick(3); K.occluded(cfg, s->ds, s->pool, r, st); ev.tick(-1); ++launches;
+    return launches + 2;
+}
+
+// The state of one render between its set-up and its tear-down: the start and stop events, the captured graph and the counts the
+// launch loop reports.  Its destructor leaves the stream idle and releases the events and the graph on every return path.
+struct RenderRun {
+    cudaStream_t st;
+    cudaEvent_t start = nullptr, stop = nullptr;
     cudaGraph_t graph = nullptr;
-    cudaGraphExec_t graphExec = nullptr;
-    guard.graph = &graph; guard.exec = &graphExec;
-    if (!useEvents) {
-        if (volpath || s->ds.nTextures || s->ds.envmap) {
+    cudaGraphExec_t exec = nullptr;
+    uint64_t iterations = 0, launches = 0;
+    ~RenderRun() {
+        cudaStreamSynchronize(st);
+        if (exec) cudaGraphExecDestroy(exec);
+        if (graph) cudaGraphDestroy(graph);
+        if (start) cudaEventDestroy(start);
+        if (stop) cudaEventDestroy(stop);
+    }
+};
+
+// Runs the iterations of a `path` / `volpath` render until the progress k_publish writes into the mapped ring shows no path alive and
+// every work item handed out; the cancel flag is read before each iteration.  The iterations replay one captured iteration (CTR_ITER,
+// advanced by k_publish, numbers them on the device) or, with flags bit3, are queued one by one and timed by `ev`.
+static int iterate(b2_scene *s, const Route &w, const DRender &r, const DFilter &filt, const Kernels &kn, StageEvents &ev, RenderRun &run) {
+    b2_ctx *ctx = s->ctx;
+    const cudaStream_t st = ctx->stream;
+    const bool graph = !ev.on;
+    auto enqueue = [&] { return enqueueIteration(s, w, r, filt, kn, ev); };
+    int perIter = 0;
+    if (graph) {
+        if (w.volpath || s->ds.nTextures || s->ds.envmap) {
             // k_volstep_lockstep (and the textured k_shade) have a deep local-memory frame: their first launch may have to grow the context's
             // local-memory pool, which is not allowed inside a stream capture.  The first iteration therefore runs as plain launches.
-            enqueueIteration();
-            launches += launchesPerIter;
-            ++iter;
+            run.launches += enqueue();
+            ++run.iterations;
         }
-        // the iteration index lives on the device (CTR_ITER, advanced by k_publish): one captured graph replays for every iteration
         CK(ctx, cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-        enqueueIteration();
-        {
-            cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-            cudaStreamIsCapturing(st, &cs);
-            const cudaError_t le = cudaPeekAtLastError();
-            if (cs != cudaStreamCaptureStatusActive || le != cudaSuccess) {
-                cudaStreamEndCapture(st, &graph);
-                cudaGetLastError();
-                return fail(ctx, B2_ERR_CUDA, std::string("graph capture of the iteration failed: ") + cudaGetErrorString(le) +
-                                              (volpath ? " (volpath), grid " + std::to_string(cfg.gridVolLockstep) : std::string(" (path)")) + ", smem " + std::to_string(cfg.traceSmem));
-            }
+        perIter = enqueue();
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        cudaStreamIsCapturing(st, &cs);
+        const cudaError_t le = cudaPeekAtLastError();
+        if (cs != cudaStreamCaptureStatusActive || le != cudaSuccess) {
+            cudaStreamEndCapture(st, &run.graph);
+            cudaGetLastError();
+            return fail(ctx, B2_ERR_CUDA, std::string("graph capture of the iteration failed: ") + cudaGetErrorString(le) +
+                                          (w.volpath ? " (volpath), grid " + std::to_string(kn.cfg.gridVolLockstep) : std::string(" (path)")) + ", smem " + std::to_string(kn.cfg.traceSmem));
         }
-        CK(ctx, cudaStreamEndCapture(st, &graph));
-        CK(ctx, cudaGraphInstantiate(&graphExec, graph, 0));
+        CK(ctx, cudaStreamEndCapture(st, &run.graph));
+        CK(ctx, cudaGraphInstantiate(&run.exec, run.graph, 0));
     }
-    volatile unsigned long long *ring = R.hRing;
-    while (!finished) {
-        if (s->cancel.load()) { status = B2_ERR_CANCELLED; break; }
+    volatile unsigned long long *ring = ctx->store->hRing;
+    uint64_t &iter = run.iterations;
+    uint64_t checked = 0;
+    for (;;) {
+        if (s->cancel.load()) return B2_ERR_CANCELLED;
         // consume published progress; never run more than B2_RING - 1 iterations ahead of the device
         for (;;) {
             while (checked < iter && ring[(checked % B2_RING) * 4] == checked + 1) {
                 const unsigned long long active = ring[(checked % B2_RING) * 4 + 1], next = ring[(checked % B2_RING) * 4 + 2];
                 ++checked;
-                if (active == 0 && next >= r.totalWork) { finished = true; break; }
+                if (active == 0 && next >= r.totalWork) return B2_OK;
             }
-            if (finished || iter - checked < (uint64_t) B2_RING - 1) break;
+            if (iter - checked < (uint64_t) B2_RING - 1) break;
             if (cudaStreamQuery(st) != cudaErrorNotReady && ring[(checked % B2_RING) * 4] != checked + 1) {
                 cudaError_t e = cudaStreamSynchronize(st);
-                if (ring[(checked % B2_RING) * 4] != checked + 1) {
-                    status = fail(ctx, B2_ERR_CUDA, std::string("render loop: device made no progress: ") + cudaGetErrorString(e == cudaSuccess ? cudaGetLastError() : e));
-                    finished = true;
-                    break;
-                }
+                if (ring[(checked % B2_RING) * 4] != checked + 1)
+                    return fail(ctx, B2_ERR_CUDA, std::string("render loop: device made no progress: ") + cudaGetErrorString(e == cudaSuccess ? cudaGetLastError() : e));
             }
         }
-        if (finished) break;
-        if (useEvents) enqueueIteration();
-        else if (cudaGraphLaunch(graphExec, st) != cudaSuccess) { status = fail(ctx, B2_ERR_CUDA, "cudaGraphLaunch failed"); break; }
-        launches += launchesPerIter;
+        if (!graph) perIter = enqueue();
+        else if (cudaGraphLaunch(run.exec, st) != cudaSuccess) return fail(ctx, B2_ERR_CUDA, "cudaGraphLaunch failed");
+        run.launches += perIter;
         ++iter;
-        if (iter > 100000000ull) { status = fail(ctx, B2_ERR_CUDA, "render loop did not terminate"); break; }
+        if (iter > 100000000ull) return fail(ctx, B2_ERR_CUDA, "render loop did not terminate");
     }
-    // pack + copy out (the guard destroys the graph and the events when this function returns)
-    CK(ctx, cudaEventRecord(evStop, st));
+}
+
+// Adds the per-stage device times of a finished render to the zeroed b2_stats::ms_* and n_*: from the CUDA events around each stage
+// (flags bit3), or from the %globaltimer stamps of the first B2_MAX_STAMPS iterations (`stamps`: flags bit2 in graph mode).
+static int stageTimes(b2_scene *s, const StageEvents &ev, bool stamps) {
+    b2_ctx *ctx = s->ctx;
+    RenderStore &R = *ctx->store;
+    b2_stats &t = s->stats;
+    float *ms[4] = {&t.ms_generate, &t.ms_extend, &t.ms_shade, &t.ms_occluded};
+    uint64_t *cnt[4] = {&t.n_generate, &t.n_extend, &t.n_shade, &t.n_occluded};
+    for (auto &te : ev.timed) {
+        float e = 0;
+        cudaEventElapsedTime(&e, s->timingEvents[te.second], s->timingEvents[te.second + 1]);
+        *ms[te.first] += e;
+        ++*cnt[te.first];
+    }
+    if (!stamps) return B2_OK;
+    const size_t nIt = (size_t) std::min<uint64_t>(t.iterations, B2_MAX_STAMPS);
+    std::vector<unsigned long long> a(nIt * 4), b(nIt * 4);
+    if (nIt) {
+        CK(ctx, cudaMemcpy(a.data(), R.dStampStart.p, nIt * 4 * 8, cudaMemcpyDeviceToHost));
+        CK(ctx, cudaMemcpy(b.data(), R.dStampEnd.p, nIt * 4 * 8, cudaMemcpyDeviceToHost));
+    }
+    double acc[4] = {0, 0, 0, 0};
+    for (size_t i = 0; i < nIt; ++i)
+        for (int k = 0; k < 4; ++k)
+            if (b[i * 4 + k] > a[i * 4 + k] && a[i * 4 + k] != ~0ull) { acc[k] += (double) (b[i * 4 + k] - a[i * 4 + k]) * 1e-6; ++*cnt[k]; }
+    for (int k = 0; k < 4; ++k) *ms[k] = (float) acc[k];
+    return B2_OK;
+}
+
+// The call path of every render: clears the film accumulators (pointing `r` at them), the counters and the cancel flag; runs loop(run),
+// the integrator's launches, between the start and stop events; packs the film into `film` (host or device) if the loop returned B2_OK;
+// synchronises once, reads the counters back and fills the b2_stats fields every integrator shares.  Returns the loop's status.
+template <typename Loop>
+static int renderCall(b2_scene *s, const b2_render_params *p, float *film, DRender &r, const Kernels &kn, uint32_t poolSize, Loop &&loop) {
+    b2_ctx *ctx = s->ctx;
+    RenderStore &R = *ctx->store;
+    const cudaStream_t st = ctx->stream;
+    const size_t nPix = (size_t) s->W * s->H;
+    CK(ctx, R.dFilmRGBA.alloc(nPix));
+    CK(ctx, R.dFilmW.alloc(nPix));
+    r.filmRGBA = R.dFilmRGBA.p; r.filmW = R.dFilmW.p;
+    CK(ctx, cudaMemsetAsync(R.dFilmRGBA.p, 0, nPix * sizeof(float4), st));
+    CK(ctx, cudaMemsetAsync(R.dFilmW.p, 0, nPix * sizeof(float), st));
+    CK(ctx, cudaMemsetAsync(s->dCounters.p, 0, CTR_COUNT * sizeof(unsigned long long), st));
+    s->cancel.store(0);
+    RenderRun run{st};
+    CK(ctx, cudaEventCreate(&run.start));
+    CK(ctx, cudaEventCreate(&run.stop));
+    CK(ctx, cudaEventRecord(run.start, st));
+    const int status = loop(run);
+    CK(ctx, cudaEventRecord(run.stop, st));
     if (status == B2_OK) {
         float *dOut = film;
         if (!p->film_on_device) {
             CK(ctx, R.dFilmOut.alloc(nPix * 5));
             dOut = R.dFilmOut.p;
         }
-        K.film_pack(cfg, R.dFilmRGBA.p, R.dFilmW.p, dOut, nPix, st);
+        kn.set.film_pack(kn.cfg, R.dFilmRGBA.p, R.dFilmW.p, dOut, nPix, st);
         if (!p->film_on_device) CK(ctx, cudaMemcpyAsync(film, dOut, nPix * 5 * sizeof(float), cudaMemcpyDeviceToHost, st));
     }
     CK(ctx, cudaStreamSynchronize(st));
@@ -920,40 +887,68 @@ extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
     std::vector<unsigned long long> ctr(CTR_COUNT);
     CK(ctx, cudaMemcpy(ctr.data(), s->dCounters.p, CTR_COUNT * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     float ms = 0;
-    cudaEventElapsedTime(&ms, evStart, evStop);
+    cudaEventElapsedTime(&ms, run.start, run.stop);
     b2_stats &t = s->stats;
     t.ms_generate = t.ms_extend = t.ms_shade = t.ms_occluded = 0;
     t.n_generate = t.n_extend = t.n_shade = t.n_occluded = 0;
-    for (auto &te : timed) {
-        float e = 0;
-        cudaEventElapsedTime(&e, s->timingEvents[te.second], s->timingEvents[te.second + 1]);
-        switch (te.first) {
-            case 0: t.ms_generate += e; ++t.n_generate; break;
-            case 1: t.ms_extend += e; ++t.n_extend; break;
-            case 2: t.ms_shade += e; ++t.n_shade; break;
-            default: t.ms_occluded += e; ++t.n_occluded; break;
-        }
-    }
-    if (timing && !useEvents) {
-        const size_t nIt = (size_t) std::min<uint64_t>(iter, B2_MAX_STAMPS);
-        std::vector<unsigned long long> a(nIt * 4), b(nIt * 4);
-        if (nIt) {
-            CK(ctx, cudaMemcpy(a.data(), R.dStampStart.p, nIt * 4 * 8, cudaMemcpyDeviceToHost));
-            CK(ctx, cudaMemcpy(b.data(), R.dStampEnd.p, nIt * 4 * 8, cudaMemcpyDeviceToHost));
-        }
-        float *ms[4] = {&t.ms_generate, &t.ms_extend, &t.ms_shade, &t.ms_occluded};
-        uint64_t *cnt[4] = {&t.n_generate, &t.n_extend, &t.n_shade, &t.n_occluded};
-        double acc[4] = {0, 0, 0, 0};
-        for (size_t i = 0; i < nIt; ++i)
-            for (int k = 0; k < 4; ++k)
-                if (b[i * 4 + k] > a[i * 4 + k] && a[i * 4 + k] != ~0ull) { acc[k] += (double) (b[i * 4 + k] - a[i * 4 + k]) * 1e-6; ++*cnt[k]; }
-        for (int k = 0; k < 4; ++k) *ms[k] = (float) acc[k];
-    }
-    t.pool_size = Q;
+    t.pool_size = poolSize;
     t.unoccluded_shadow_rays = ctr[CTR_UNOCCLUDED];
     t.samples = ctr[CTR_SAMPLES]; t.rays = ctr[CTR_RAYS]; t.shadow_rays = ctr[CTR_SHADOWRAYS]; t.path_length_sum = ctr[CTR_PATHLEN];
-    t.bad_samples = ctr[CTR_BAD]; t.dim_overflow = ctr[CTR_DIMOVF]; t.iterations = iter; t.kernel_launches = launches + 1;
+    t.bad_samples = ctr[CTR_BAD]; t.dim_overflow = ctr[CTR_DIMOVF]; t.iterations = run.iterations; t.kernel_launches = run.launches + 1;
     t.ms_total = ms;
+    return status;
+}
+
+// `direct`: k_direct over the work items in slices of whole samples of the film, so that b2_cancel is honoured between launches; no
+// path pool, and every launch counts as an iteration.  k_direct never adds to CTR_PATHLEN, so path_length_sum stays 0.
+static int directSlices(b2_scene *s, const DRender &r, const DFilter &filt, const Kernels &kn, RenderRun &run) {
+    const cudaStream_t st = s->ctx->stream;
+    // a slice: enough whole samples of the film for ~16M items (a few ms on the flat route), at least one sample; the cancel flag is
+    // read before each launch
+    const uint64_t perSample = (uint64_t) s->W * s->H, nS = (uint64_t) (r.sampleHi - r.sampleLo);
+    const uint64_t slice = perSample * std::max<uint64_t>(1, std::min<uint64_t>(nS, (16ull << 20) / std::max<uint64_t>(1, perSample)));
+    int status = B2_OK;
+    for (uint64_t b = 0; b < r.totalWork; b += slice) {
+        if (s->cancel.load()) { status = B2_ERR_CANCELLED; break; }
+        if (run.launches >= 2) cudaStreamSynchronize(st); // from the third slice on, the host waits for the queued ones: a cancel waits for at most two slices, not for the render
+        kn.set.direct(kn.cfg, s->ds, r, filt, s->dCounters.p, b, std::min(r.totalWork, b + slice), st);
+        run.iterations = ++run.launches;
+    }
+    CK(s->ctx, cudaGetLastError());
+    return status;
+}
+
+extern "C" int b2_render(b2_scene *s, const b2_render_params *p, float *film) {
+    if (!s || !p || !film) return fail(s ? s->ctx : nullptr, B2_ERR_INVALID, "b2_render: null argument");
+    b2_ctx *ctx = s->ctx;
+    if (!s->committed) return fail(ctx, B2_ERR_INVALID, "b2_render: scene not committed");
+    CK(ctx, cudaSetDevice(ctx->device));
+    std::lock_guard<std::mutex> renderLock(ctx->store->renderMutex);
+    DRender r;
+    if (int rc = fillRender(s, p, r)) return rc;
+    DFilter filt;
+    if (int rc = makeFilter(ctx, p->rfilter, p->rfilter_param, filt)) return rc;
+    // Which kernel set renders?  parity_mode 1: the IEEE build (-fmad=false, accurate division / sqrt / sincos, TriAccel).  parity_mode 0: the
+    // throughput build -- EXCEPT for `path` renders of scenes with a transmissive BSDF.  A path that bounces inside a glass ball amplifies
+    // ulp-level differences chaotically: under FMA contraction alone a few in 1e5 of such paths leave the reference's path (different hit,
+    // other lobe, other ending -- not fast-math, not the plane-form triangle test), each an unrelated sample of a heavy-tailed estimator,
+    // i.e. above 1e-3 relative L2 at 1024^2 @ 512 spp whatever else the kernels do.  Shading such scenes
+    // with the IEEE kernels and keeping only the traversal fast ("hybrid", tried: exact TriAccel (t,u,v) of the winning triangle) removes
+    // a third of the flips -- the fast traversal still picks the neighbouring triangle at shared edges -- so those scenes get the IEEE
+    // build as a whole (BVH traversal dominates BASELINE config 3, so the IEEE shading costs little there).  flags bit8 forces the throughput kernels.
+    const bool autoIeee = s->hasTransmission && p->integrator == B2_INTEGRATOR_PATH && !(p->flags & 256);
+    const bool parityMode = p->parity_mode != 0 || autoIeee;
+    const Kernels kn = kernelsFor(s, parityMode);
+    if (p->integrator == B2_INTEGRATOR_DIRECT)
+        return renderCall(s, p, film, r, kn, 0, [&](RenderRun &run) { return directSlices(s, r, filt, kn, run); });
+    if (int rc = diagnosticBuffers(s, p, r)) return rc;
+    const Route w = chooseRoute(s, p, r);
+    if (int rc = ensurePool(s, w.Q, w.volpath, r)) return rc;
+    const bool useEvents = (p->flags & 8) != 0; // no graph: plain launches bracketed by CUDA events (cross-check path)
+    StageEvents ev{s, useEvents};
+    const int status = renderCall(s, p, film, r, kn, w.Q, [&](RenderRun &run) { return iterate(s, w, r, filt, kn, ev, run); });
+    if (status != B2_OK && status != B2_ERR_CANCELLED) return status; // the stats may still be those of the render before
+    if (int rc = stageTimes(s, ev, (p->flags & 4) && !useEvents)) return rc;
     return status;
 }
 
